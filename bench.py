@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """bench.py -- frames/s of the splat render hot path (preprocess | sort | blend).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3] [--dump-outputs DIR]
 
 A "step" is one frame: GaussianRenderer.prepare + render of one camera of the 36-view orbit
 (BASELINE.md section 3) over a synthetic cloud that is already resident in HBM (PointCloud::new is
 load-time in the reference too, pointcloud.rs:99).  Default workload = cfg3, the configuration
-BASELINE.json's metric and target are quoted on: 6M Gaussians, 1920x1080, SH degree 3, 1xB200.
+BASELINE.json's metric and target are quoted on: 6M Gaussians, 1920x1080, SH degree 3, 1xH100.
 
   value  frames/s over exactly K frames, CUDA events on the launching stream, frame written to a
-         device target (inputs resident; the 744 MB cloud is ~6x the 126 MB L2, so nothing
+         device target (inputs resident; the 744 MB cloud is ~15x the 50 MB L2, so nothing
          survives in L2 between frames)
   e2e    the same K frames through the public API with HOST buffers: per frame the camera/settings
          uniforms go host->device and the finished RGBA16F frame comes back into pinned host memory
@@ -17,7 +17,9 @@ BASELINE.json's metric and target are quoted on: 6M Gaussians, 1920x1080, SH deg
   cpu_baseline         the CPU oracle (port of the reference algorithm; the reference itself is
                        Rust+WGSL on wgpu/Vulkan and cannot run here) timed on one frame
 
---impl reference runs that CPU oracle as the reference arm (oracle/_ref cannot be built).
+--impl reference runs that CPU oracle as the reference arm (oracle/_ref cannot be built): --warmup W
+untimed frames, then exactly K timed frames (a CPU frame of cfg3 takes seconds: choose K accordingly).
+--dump-outputs DIR writes the frame the last timed step rendered (see dump_outputs).
 """
 import argparse
 import json
@@ -34,9 +36,10 @@ if ROOT not in sys.path:
 import numpy as np  # noqa: E402
 
 METRIC = "frames/sec"
-REFERENCE_BUDGET_S = 120.0                  # host seconds the reference arm may spend on timed frames
 KERNELS_STAGE1 = 3                          # count, scan, preprocess
 KERNELS_BINNING = 3                         # count, scan, expand (per slab; the tile ranges are fused into the last onesweep pass)
+DUMP_LIMIT = 64 << 20                       # bytes --dump-outputs may write
+DUMP_SAMPLE_PIXELS = 1 << 20                # pixels kept of a frame above DUMP_LIMIT (fixed seed)
 
 
 def measured_peaks():
@@ -47,11 +50,11 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1965.0))
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0
+    return 3350.0, "fallback (H100 SXM data sheet, not measured)", 1980.0
 
 
 class ClockSampler(threading.Thread):
-    """SM clock + throttle reasons during the timed region (B200_PROFILING.md recipe), sampled through
+    """SM clock + throttle reasons during the timed region, sampled through
     NVML every 10 ms (the nvidia-smi CLI takes ~100 ms per query, longer than a whole timed region)."""
 
     def __init__(self, index):
@@ -117,6 +120,21 @@ def frame_crc(host):
 CHECKSUM_VIEW = 0                           # index into the workload's camera list
 
 
+def dump_outputs(out_dir, frame):
+    """Write `frame` (the device target the last timed step rendered into) as float32 (exact for RGBA16F).  A frame above
+    DUMP_LIMIT is written as a fixed, seeded sample of its pixels (frame_sample.npy, [n, 4]) with their row-major pixel
+    indices (frame_sample_index.npy, float64: exact below 2^53), so two builds can be compared pixel for pixel."""
+    os.makedirs(out_dir, exist_ok=True)
+    img = frame.float().cpu().numpy()
+    if img.nbytes <= DUMP_LIMIT:
+        np.save(os.path.join(out_dir, "frame.npy"), img)
+        return
+    px = img.reshape(-1, img.shape[-1])
+    idx = np.sort(np.random.default_rng(0).choice(len(px), size=min(DUMP_SAMPLE_PIXELS, len(px)), replace=False))
+    np.save(os.path.join(out_dir, "frame_sample.npy"), px[idx])
+    np.save(os.path.join(out_dir, "frame_sample_index.npy"), idx.astype(np.float64))
+
+
 def host_threads():
     """host cores this process may use (affinity / cgroup aware); the oracle legs set their OpenMP count from it --
     torchrun exports OMP_NUM_THREADS=1 to every rank, which would otherwise shrink the reference arm to one core"""
@@ -129,7 +147,14 @@ def host_threads():
 def make_workload(name):
     import websplat_b200 as ws
     n, W, H, seed, compressed = ws.synth.CONFIGS[name]
-    cache = os.path.join("/tmp", "ws_cloud_%s.npz" % name)
+    # Raw clouds take tens of seconds to generate at cfg3, so they are cached in the temporary directory under a name that
+    # carries the generator's source hash and the configuration (and the user, so no other user's file is ever read):
+    # a cache written by a different generator or configuration can never be picked up.
+    import hashlib
+    import tempfile
+    with open(ws.synth.__file__, "rb") as f:
+        key = hashlib.sha256(f.read() + repr(ws.synth.CONFIGS[name]).encode()).hexdigest()[:16]
+    cache = os.path.join(tempfile.gettempdir(), "ws_cloud_%s_%d_%s.npz" % (name, os.getuid(), key))
     cloud = None
     if os.path.exists(cache):
         try:
@@ -144,8 +169,10 @@ def make_workload(name):
     if cloud is None:
         cloud = ws.synth.make_cloud_compressed(n, seed) if compressed else ws.synth.make_cloud(n, seed)
         if not compressed:
-            try:
-                np.savez(cache, **{k: (v.view(np.uint8) if k == "gaussians" else v) for k, v in cloud.items()})
+            try:                                   # written under a private name, then renamed: readers never see a partial file
+                tmp = "%s.%d.tmp.npz" % (cache[:-4], os.getpid())
+                np.savez(tmp, **{k: (v.view(np.uint8) if k == "gaussians" else v) for k, v in cloud.items()})
+                os.replace(tmp, cache)
             except Exception:
                 pass
     views = [ws.synth.fixed_camera()] if name == "cfg1" else ws.synth.orbit_views(36)
@@ -184,21 +211,9 @@ def run_reference(args):
     from oracle import oracle as orc
     orc.build()
     orc.set_num_threads(host_threads())
-    # The driver launches this arm with the GPU arm's --steps / --warmup (hundreds of steps); a CPU frame of cfg3 takes
-    # seconds.  The sample is therefore bounded: at most 3 warm-up frames, then as many FULL frames of the orbit as fit
-    # REFERENCE_BUDGET_S (never fewer than 1, never more than --steps); `steps` reports the frames actually timed.
-    t_frame = None
-    for i in range(min(args.warmup, 3)):
-        t1 = time.perf_counter()
+    # exactly --warmup untimed frames, then exactly --steps timed FULL frames of the orbit
+    for i in range(args.warmup):
         oracle_frame_seconds(cloud, views[i % len(views)], W, H)
-        t_frame = time.perf_counter() - t1
-    if t_frame is None:
-        t1 = time.perf_counter()
-        oracle_frame_seconds(cloud, views[0], W, H)
-        t_frame = time.perf_counter() - t1
-    timed = max(1, min(args.steps, int(REFERENCE_BUDGET_S / max(t_frame, 1e-6))))
-    requested = args.steps
-    args.steps = timed
     t0 = time.perf_counter()
     for i in range(args.steps):
         oracle_frame_seconds(cloud, views[i % len(views)], W, H)
@@ -207,14 +222,13 @@ def run_reference(args):
     cores = orc.num_threads()
     line = {
         "impl": "reference", "metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": args.gpus,
-        "steps": args.steps, "warmup": max(1, min(args.warmup, 3)), "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True,
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload_name(args.workload, cloud, W, H), "views": len(views),
-                   "steps_requested": requested, "warmup_requested": args.warmup},
+                   "steps_requested": args.steps, "warmup_requested": args.warmup},
         "cpu_baseline": {"value": fps, "unit": "frames/s", "cores": cores, "kind": "port",
-                         "sample": "%d full frames of the same workload on the CPU oracle (OpenMP, %d threads; %d steps were requested, "
-                                   "the sample is bounded to ~%d s of host time); the reference itself (Rust+WGSL on wgpu/Vulkan) "
-                                   "cannot be built or run on this box" % (args.steps, cores, requested, int(REFERENCE_BUDGET_S))},
+                         "sample": "%d full frames of the same workload on the CPU oracle (OpenMP, %d threads); the reference "
+                                   "itself (Rust+WGSL on wgpu/Vulkan) cannot be built or run on this box" % (args.steps, cores)},
         "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
     }
@@ -253,7 +267,7 @@ def run_ours(args):
     pc = ws.PointCloud.new(ctx, gen)
     # `depth` frames in flight: one renderer (own scratch) + one stream + one target per frame slot, all reading the
     # same resident cloud; frame i runs in slot i % depth.  At the small configurations one frame's kernels are
-    # latency-bound and a second frame fills the idle SMs (cfg1 +36 %, cfg2 +22 %, cfg3 +2 %: profiles/r01o_*).
+    # latency-bound and a second frame fills the idle SMs.
     depth = int(args.frames_in_flight) if args.frames_in_flight > 0 else 2
     split_req = False if args.no_occlusion_split else None        # None = the library's automatic choice (on from 2 M points)
     split = (not args.no_occlusion_split) and cloud["num_points"] >= 2_000_000
@@ -303,6 +317,8 @@ def run_ours(args):
     ms_total = e0.elapsed_time(e1)
     clocks = sampler.finish()
     fps = K / (ms_total * 1e-3)
+    if args.dump_outputs:                      # before the e2e section below reuses the targets
+        dump_outputs(args.dump_outputs, targets[(Wu + K - 1) % depth])
 
     # ---- e2e: host buffers, uniforms H2D + frame D2H inside the timed region ----------------------
     # The public API is asynchronous on the caller's stream, so a caller that wants throughput keeps
@@ -403,42 +419,19 @@ def run_ours(args):
     sb_bytes = depth_passes * V * 16 + V * 12 + P * 8 + tile_passes * P * 16 + T * 8 + P * 24 + T * 8 + W * H * bpp
     sb_bytes_full = depth_passes * V * 16 + V * 12 + P_full * 8 + tile_passes * P_full * 16 + T * 8 + P_full * 24 + T * 8 + W * H * bpp
     dom = max(kernels, key=lambda k_: kernels[k_]["ms"] * kernels[k_].get("launches", 1))
-    # DRAM traffic of the dominant kernel (same unit of work as its `bytes`) from the committed ncu --set full captures (cfg3 only)
-    traffic, traffic_src = None, None
-    try:
-        if args.workload == "cfg3" and split:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "kernel_traffic_cfg3_split.json")))
-            traffic = tj["per_stage"][dom]["dram_bytes"]
-            traffic_src = "profiles/kernel_traffic_cfg3_split.json (%s; %s)" % (tj.get("source", "ncu --set full"), tj["per_stage"][dom]["launches"])
-        elif args.workload == "cfg3":
-            tj = json.load(open(os.path.join(ROOT, "profiles", "kernel_traffic_cfg3.json")))
-            key = {"composite": "composite_kernel<1>", "preprocess": "preprocess_kernel<0>", "binning": "bin_expand_kernel",
-                   "tile_sort_pass": "onesweep_pass_kernel<1>", "depth_sort_pass": "onesweep_pass_kernel<0>"}[dom]
-            traffic = tj[key]["dram_bytes_per_launch"]
-            traffic_src = "profiles/kernel_traffic_cfg3.json (ncu --set full, r01m, one-pass frame)"
-    except Exception:
-        traffic = None
-    # measured issue / pipe utilisation of the compositor (ncu capture committed under profiles/; None until one exists)
-    pipes, pipes_src = None, None
-    try:
-        pj = json.load(open(os.path.join(ROOT, "profiles", "composite_pipes_%s.json" % args.workload)))
-        pipes, pipes_src = pj.get("metrics"), pj.get("source")
-    except Exception:
-        pass
     sb_ms = acc["ms_sort"] + acc["ms_blend"]
     roofline = {
         "kernel": dom, "bound": "hbm", "achieved": kernels[dom]["gbs"], "peak": peak, "unit": "GB/s",
         "frac": kernels[dom]["frac"], "frac_full_pairs": kernels[dom].get("frac_full_pairs"),
-        "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+        "peak_source": peak_src,
         "bytes_formula": "SURVEY.md 8(d): blend = P*(4+20) + T*8 + W*H*B_fmt with P = pairs emitted; no state round trip",
         "note": "stage 3 is FP32/MUFU-issue bound, not HBM bound (SURVEY 8(d)); its HBM fraction is reported because "
-                "the north star asks for it; 'composite_pipes' holds the measured issue / pipe utilisation (ncu). `frac` prices the "
+                "the north star asks for it. `frac` prices the "
                 "pairs actually EMITTED (%.1f M of the %.1f M of the complete list: the occlusion split drops the rest before they "
                 "are sorted), so it falls when the split removes bytes faster than time; `frac_full_pairs` prices the same time at "
                 "the complete pair list" % (P / 1e6, P_full / 1e6),
         "sort_plus_blend": {"bytes": sb_bytes, "ms": sb_ms, "gbs": gbs(sb_bytes, sb_ms), "frac": gbs(sb_bytes, sb_ms) / peak,
                             "frac_full_pairs": gbs(sb_bytes_full, sb_ms) / peak},
-        "composite_pipes": pipes, "composite_pipes_source": pipes_src,
     }
 
     # ---- extra lines (not the headline): the reference's `measure` protocol and the CUB yard-stick ---------------
@@ -468,10 +461,6 @@ def run_ours(args):
             del rm, mt
         except Exception as e:                         # never lose the headline to an extra
             extra["measure_equivalent"] = {"error": str(e)[:200]}
-        try:
-            extra["sort_vs_cub"] = json.load(open(os.path.join(ROOT, "profiles", "r02_sort_vs_cub.json")))
-        except Exception:
-            pass
 
     # ---- CPU baseline: one frame of the same workload on the host cores -------------------------
     cpu = None
@@ -485,7 +474,7 @@ def run_ours(args):
         "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload_name(args.workload, cloud, W, H), "target_format": "rgba16float",
-                   "l2": "inputs (%.0f MB cloud) larger than the 126 MB L2; no flush needed" % ((cloud["gaussians"].nbytes + cloud["sh_coefs"].nbytes) / 1e6),
+                   "l2": "inputs (%.0f MB cloud) larger than the 50 MB L2; no flush needed" % ((cloud["gaussians"].nbytes + cloud["sh_coefs"].nbytes) / 1e6),
                    "frames_in_flight": depth,
                    "occlusion_split": ("two depth slabs, the far one culled against the tiles the near one saturated: P_mean counts "
                                        "the pairs actually emitted; the image is bit-identical to the one-pass frame") if split else "off",
@@ -521,9 +510,15 @@ def main():
                          "(the smaller the per-GPU share, the more latency-bound a single frame is)")
     ap.add_argument("--no-occlusion-split", action="store_true", help="single-GPU arm: bin / tile-sort / composite all pairs in one pass")
     ap.add_argument("--equal-bands", action="store_true", help="multi-GPU arm: keep the equal tile-row split instead of cost-balanced bands")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the frame the last timed step rendered to DIR/*.npy (float32; a seeded pixel sample above 64 MB)")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 360 if args.impl == "ours" else 10    # 10 orbits (~1 s of GPU time) / ~2-5 s per CPU frame
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
+    if args.dump_outputs and (args.impl != "ours" or args.gpus != 1):
+        ap.error("--dump-outputs is supported with --impl ours --gpus 1")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

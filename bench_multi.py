@@ -60,10 +60,9 @@ def run(args):
     depth = int(getattr(args, "frames_in_flight", 0) or 0)
     if depth <= 0:
         # the smaller a GPU's share, the more latency-bound a single frame is and the more frames fit next to each other.
-        # Measured on cfg3 (profiles/r02h_*, r02j_*, 108 timed frames): 8 GPUs 3107* (3 in flight) / 3275 (4) / 3414 (5) / 3357 (6) /
-        # 3366 (8) frames/s; 4 GPUs 1843** (2) / 2080 (3) / 2102 (4); 2 GPUs 1264** (2) / 1363 (3) / 1338 (4).  A deeper pipeline
-        # also ramps up longer, which a 20-frame run sees (8 GPUs, 20 frames: 3107 with 3 in flight, 2920 with 6), hence 4 at 8 GPUs.
-        # (* 20 frames; ** before the near-slab / sampler changes of the same round)
+        # The depths come from a sweep of 2-8 frames in flight at cfg3 on 2, 4 and 8 GPUs of the previous target GPU;
+        # they have not been re-measured on H100.  A deeper pipeline also ramps up
+        # longer, which a short run sees, hence 4 at 8 GPUs.
         depth = 4 if world >= 8 else 3
     pipe = ws.ShardedPipeline(ws, ctx, fmt, cloud["sh_deg"], cloud["compressed"], pc, N, (W, H), depth=depth,
                               pair_capacity=min(max(8 * N // world + (1 << 22), 1 << 22), (1 << 30) - 1))
@@ -107,7 +106,7 @@ def run(args):
     if rank == 0:
         checksum = bench.frame_crc(chk)
         if args.workload == "cfg5":
-            # cfg5 exists only sharded; the union of the ranks' shards IS the cloud (24 M fits one B200): rebuild it here
+            # cfg5 exists only sharded; the union of the ranks' shards IS the cloud (24 M fits one H100): rebuild it here
             parts = [shard if q == 0 else ws.synth.make_cloud((n_all * (q + 1)) // world - (n_all * q) // world, seed + 7919 * q, density_n=n_all)
                      for q in range(world)]
             full = dict(cloud, gaussians=np.concatenate([p_["gaussians"] for p_ in parts]),
@@ -207,7 +206,7 @@ def run(args):
                              "note": "max over ranks of each stage", "phases_rank0": phases},
             "roofline": {"kernel": "sort+blend (all ranks)", "bound": "hbm", "achieved": bytes_sort_blend / (sb_ms * 1e-3) / 1e9 if sb_ms > 0 else 0.0,
                          "peak": peak * world, "unit": "GB/s", "frac": (bytes_sort_blend / (sb_ms * 1e-3) / 1e9) / (peak * world) if sb_ms > 0 else 0.0,
-                         "traffic": None, "peak_source": peak_src + " x n_gpus"},
+                         "peak_source": peak_src + " x n_gpus"},
             "cpu_baseline": None,
             "e2e": {"value": K / e2e_s, "unit": "frames/s", "h2d_bytes_per_step": 480 * world, "d2h_bytes_per_step": W * H * 8,
                     "checksum": checksum, "checksum_what": "CRC-32 of the full RGBA16F frame of view %d, assembled from the %d ranks' bands and downloaded on rank 0" % (bench.CHECKSUM_VIEW, world),

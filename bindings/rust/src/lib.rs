@@ -1,4 +1,4 @@
-//! Drop-in for web-splat's render path on a B200: the reference's `PointCloud`, `SplattingArgs` and
+//! Drop-in for web-splat's render path on an H100: the reference's `PointCloud`, `SplattingArgs` and
 //! `GaussianRenderer::{new, prepare, render, num_visible_points, color_format}` (src/pointcloud.rs:72-349,
 //! src/renderer.rs:33-260,587-599) on top of libwebsplat_b200.so.  SOURCE ONLY -- see Cargo.toml.
 //!

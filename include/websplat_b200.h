@@ -1,5 +1,5 @@
 /*
- * websplat_b200.h -- C ABI of the B200-native splat render path.
+ * websplat_b200.h -- C ABI of the H100-native (sm_90a) splat render path.
  *
  * This is the drop-in boundary for the ONE hot path of KeKsBoTer/web-splat:
  * GaussianRenderer::prepare + GaussianRenderer::render and the PointCloud GPU
@@ -19,7 +19,7 @@
  *  - a ws_renderer is not re-entrant (same as `&mut self` in renderer.rs:191):
  *    one host thread per renderer handle, frames serialised by the caller.
  *  - there is no CPU fallback: every entry point that does work needs a CUDA
- *    device of compute capability 10.x and fails with WS_ERR_CUDA otherwise.
+ *    device of compute capability 9.0 (sm_90a, H100) and fails with WS_ERR_CUDA otherwise.
  */
 #ifndef WEBSPLAT_B200_H
 #define WEBSPLAT_B200_H

@@ -24,7 +24,7 @@
  * implementation, so this file fixes ONE conforming evaluation: dot products
  * and matrix products accumulate with fmaf(), and a quotient whose divisor is
  * shared (x/w, y/w, z/w; J's 1/z; normalize) is formed as a correctly rounded
- * reciprocal times the numerator.  The sm_100a kernels mirror it operation for
+ * reciprocal times the numerator.  The sm_90a kernels mirror it operation for
  * operation (FFMA / MUFU.RCP + Newton = __frcp_rn), which is what keeps stage 1
  * bit-exact between the two while costing ~20 % fewer instructions than the
  * round-1 "one rounding per written operation" form.

@@ -1,5 +1,5 @@
-// Microbenchmark: cost of warp-level digit matching / histogram primitives on sm_100a.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o rank_primitives rank_primitives.cu && ./rank_primitives
+// Microbenchmark: cost of warp-level digit matching / histogram primitives on sm_90a.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o rank_primitives rank_primitives.cu && ./rank_primitives
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -62,7 +62,7 @@ __global__ void bench(uint32_t *out, int iters, uint32_t distinct_mask, long lon
 }
 
 template <int MODE>
-void run(const char *name, uint32_t mask, uint32_t *out, long long *cyc, int blocks, int threads)
+void run(const char *name, uint32_t mask, uint32_t *out, long long *cyc, int blocks, int threads, int sms)
 {
     const int iters = 2000;
     cudaMemset(cyc, 0, 8);
@@ -76,22 +76,25 @@ void run(const char *name, uint32_t mask, uint32_t *out, long long *cyc, int blo
     long long c; cudaMemcpy(&c, cyc, 8, cudaMemcpyDeviceToHost);
     const double warp_ops = (double)blocks * (threads / 32) * iters;
     printf("%-44s mask %02x  blocks/SM %d x %d thr: %7.2f cycles/op/CTA-clock  %8.2f Gwarp-op/s  (%.3f ms)\n", name, mask,
-           blocks / 148, threads, (double)c / blocks / iters, warp_ops / (ms * 1e6), ms);
+           blocks / sms, threads, (double)c / blocks / iters, warp_ops / (ms * 1e6), ms);
 }
 
 int main()
 {
+    cudaDeviceProp prop;
+    cudaGetDeviceProperties(&prop, 0);
+    const int sms = prop.multiProcessorCount;          // one full wave per occupancy level, whatever the chip
     uint32_t *out; long long *cyc;
-    cudaMalloc(&out, 148 * 8 * 256 * 4); cudaMalloc(&cyc, 8);
+    cudaMalloc(&out, (size_t)sms * 8 * 256 * 4); cudaMalloc(&cyc, 8);
     for (int occ : {1, 4, 8}) {
-        const int blocks = 148 * occ, threads = 256;
+        const int blocks = sms * occ, threads = 256;
         for (uint32_t mask : {0xffu, 0x0fu, 0x01u}) {
-            run<0>("MATCH.ANY", mask, out, cyc, blocks, threads);
-            run<1>("8x BALLOT peers", mask, out, cyc, blocks, threads);
-            run<2>("smem atomicAdd (no return)", mask, out, cyc, blocks, threads);
-            run<5>("smem atomicAdd (return)", mask, out, cyc, blocks, threads);
-            run<3>("ballot peers + leader RMW + shfl (rank)", mask, out, cyc, blocks, threads);
-            run<4>("MATCH.ANY + leader atomicAdd + shfl (rank)", mask, out, cyc, blocks, threads);
+            run<0>("MATCH.ANY", mask, out, cyc, blocks, threads, sms);
+            run<1>("8x BALLOT peers", mask, out, cyc, blocks, threads, sms);
+            run<2>("smem atomicAdd (no return)", mask, out, cyc, blocks, threads, sms);
+            run<5>("smem atomicAdd (return)", mask, out, cyc, blocks, threads, sms);
+            run<3>("ballot peers + leader RMW + shfl (rank)", mask, out, cyc, blocks, threads, sms);
+            run<4>("MATCH.ANY + leader atomicAdd + shfl (rank)", mask, out, cyc, blocks, threads, sms);
         }
     }
     return 0;

@@ -6,7 +6,7 @@
 // Both sorts are stable LSD radix sorts, so the outputs must be bit-identical: checked here.
 //
 // build (done by profiles/microbench/build.sh):
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I web-splat_b200/csrc -I include \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I web-splat_b200/csrc -I include \
 //        profiles/microbench/sort_vs_cub.cu web-splat_b200/build/radix_sort.o -o profiles/microbench/sort_vs_cub
 // run:  WS_SORT_VARIANT=2 ./sort_vs_cub   (1 = the round-1 pass)
 #include <cub/cub.cuh>

@@ -1,5 +1,5 @@
 """Offline dataset renderer: `python scripts/render_scene.py <input.ply|.npz> <cameras.json> <img_out> [--max-sh-deg N]`.
-The B200 counterpart of the reference's `render` binary (bin/render.rs:14-180): renders the test split, then the
+The CUDA counterpart of the reference's `render` binary (bin/render.rs:14-180): renders the test split, then the
 train split, of a 3DGS cameras.json to PNG files."""
 import argparse
 import os

@@ -53,7 +53,7 @@ def test_status_strings_and_version(ws):
     L = ws.lib()
     assert L.ws_status_string(0) == b"ok"
     assert b"pair" in L.ws_status_string(ws.WS_ERR_PAIR_OVERFLOW)
-    assert b"sm_100a" in L.ws_version()
+    assert b"sm_90a" in L.ws_version()
 
 
 def test_no_cpu_fallback_without_gpu(ws):

@@ -68,3 +68,48 @@ def test_frame_crc_is_a_full_frame_hash():
         b = a.copy(); b[y, x, ch] = np.float16(6.1e-5)
         assert bench.frame_crc(b) != c0
     assert bench.frame_crc(a.copy()) == c0 and len(c0) == 8
+
+
+def test_reference_arm_times_exactly_the_requested_steps():
+    """--steps is the number of timed frames and --warmup the number of untimed ones, on the reference arm too"""
+    p = _run("--impl", "reference", "--workload", "cfg1", "--steps", "7", "--warmup", "5")
+    assert p.returncode == 0, p.stderr[-2000:]
+    d = json.loads(p.stdout.strip().splitlines()[-1])
+    assert d["steps"] == 7 and d["warmup"] == 5 and d["config"]["steps_requested"] == 7
+    assert abs(d["ms_per_step"] * d["value"] - 1000.0) < 1.0 and "7 full frames" in d["cpu_baseline"]["sample"]
+
+
+def test_steps_below_one_are_rejected():
+    for argv in (("--steps", "0"), ("--impl", "reference", "--steps", "0"), ("--steps", "2", "--warmup", "-1")):
+        p = _run(*argv)
+        assert p.returncode == 2 and "--steps must be at least 1" in p.stderr, (argv, p.stderr[-500:])
+
+
+def test_dump_outputs_writes_the_frame_or_a_fixed_sample_under_64_mb(tmp_path):
+    """--dump-outputs: the cfg3 frame (33 MB as float32) is written whole; the cfg4 frame (133 MB) as a seeded pixel sample
+    with its row-major indices; float dtypes only, at most 64 MB, and the same bytes every time"""
+    import numpy as np
+    import torch
+    sys.path.insert(0, ROOT)
+    import bench
+    g = torch.Generator().manual_seed(3)
+    for (H, W), names in (((1080, 1920), ["frame.npy"]), ((2160, 3840), ["frame_sample.npy", "frame_sample_index.npy"])):
+        frame = torch.rand((H, W, 4), generator=g).to(torch.float16)
+        outs = []
+        for run in range(2):
+            d = tmp_path / ("%dx%d_%d" % (W, H, run))
+            bench.dump_outputs(str(d), frame)
+            assert sorted(os.listdir(d)) == sorted(names)
+            assert sum(os.path.getsize(d / n) for n in names) <= 64 << 20
+            outs.append({n: (d / n).read_bytes() for n in names})
+        assert outs[0] == outs[1]
+        full = frame.float().numpy()
+        if names == ["frame.npy"]:
+            a = np.load(tmp_path / ("%dx%d_0" % (W, H)) / "frame.npy")
+            assert a.dtype == np.float32 and np.array_equal(a, full)
+        else:
+            d = tmp_path / ("%dx%d_0" % (W, H))
+            px, idx = np.load(d / "frame_sample.npy"), np.load(d / "frame_sample_index.npy")
+            assert px.dtype == np.float32 and idx.dtype == np.float64 and px.shape == (len(idx), 4)
+            assert len(idx) == bench.DUMP_SAMPLE_PIXELS and (np.diff(idx) > 0).all()
+            assert np.array_equal(px, full.reshape(-1, 4)[idx.astype(np.int64)])

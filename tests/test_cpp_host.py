@@ -91,8 +91,7 @@ def test_cpp_tool_errors(ws, tool, tmp_path):
 
 @pytest.mark.gpu
 def test_gpu_cpp_tool_renders_like_the_python_tool(ws, ctx, tool, tmp_path):
-    """the C++ host mirror + offline tool on a GPU: PNG for PNG what scripts/render_scene.py writes
-    (first run on a B200: round 2, profiles/r02b_pytest_gpu.log)"""
+    """the C++ host mirror + offline tool on a GPU: PNG for PNG what scripts/render_scene.py writes"""
     n, W, H = 20000, 320, 200
     ply = tmp_path / "cloud.ply"; ply.write_bytes(ws.synth.ply_bytes(ws.synth.ply_vertices(n, 8, 3), 3))
     cams = tmp_path / "cameras.json"; cams.write_text(json.dumps(_scene_entries(ws, 9, W, H)))

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path, called through the C ABI, against the CPU oracle.
+"""GPU parity tests: the sm_90a path, called through the C ABI, against the CPU oracle.
 
 Bars (DESIGN.md "Parity"):
   stage 1 raw layout      bit-exact (visible set, 10 halves, depth key, tile rect, V, P)

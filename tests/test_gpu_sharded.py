@@ -1,6 +1,6 @@
 """GPU tests of the sharded path.  world == 1 exercises the whole begin/exchange/finish/band sequence
-on one GPU (the exchange then stores into local memory); the 2-GPU test runs under
-`gpurun --gpus 2` and checks that the 2-GPU frame is BIT-IDENTICAL to the 1-GPU frame."""
+on one GPU (the exchange then stores into local memory); the multi-GPU tests run on
+2, 4 or 8 GPUs and check that the 2-GPU frame is BIT-IDENTICAL to the 1-GPU frame."""
 import os
 import subprocess
 import sys
@@ -81,10 +81,10 @@ def _gpu_count():
 def test_sharded_frames_bit_identical_to_one_gpu(world):
     """SURVEY.md 8(e): G in {1, 2, 4, 8} images bit-identical.  tests/sharded_worker.py renders the same frames on `world`
     GPUs (all three exchange variants, two frames in flight over re-cut bands, a cfg5-style cloud whose shards are
-    generated per rank) and on one GPU and requires torch.equal.  Needs `world` GPUs: `gpurun --gpus N`; the log of the
-    8-GPU run is committed under profiles/."""
+    generated per rank) and on one GPU and requires torch.equal.  Needs `world` GPUs; WS_SHARDED_LOG_DIR keeps the
+    workers' log."""
     if _gpu_count() < world:
-        pytest.skip("needs %d GPUs (gpurun --gpus %d)" % (world, world))
+        pytest.skip("needs %d GPUs" % world)
     env = dict(os.environ, PYTHONPATH=ROOT)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=%d" % world, "--master-addr", "127.0.0.1",
            "--master-port", str(29517 + world), os.path.join(ROOT, "tests", "sharded_worker.py")]

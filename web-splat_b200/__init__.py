@@ -18,7 +18,7 @@ C ABI is mirrored here with the SAME names, argument meaning and error behaviour
     num_visible_points             renderer.rs:170     GaussianRenderer.num_visible_points()
     GPUStopwatch                   utils.rs:26-134     GaussianRenderer.stats()
 
-This module is plumbing only: every frame is produced by the hand-written sm_100a kernels in
+This module is plumbing only: every frame is produced by the hand-written sm_90a kernels in
 csrc/ through libwebsplat_b200.so.  There is NO CPU fallback: if the library is missing it
 is built with nvcc; if no CUDA device is present Context() raises.
 """
@@ -150,7 +150,7 @@ _lib = None
 
 
 def build_library(force=False):
-    """Compile libwebsplat_b200.so in-tree with nvcc (sm_100a).  No fallback if nvcc fails."""
+    """Compile libwebsplat_b200.so in-tree with nvcc (sm_90a).  No fallback if nvcc fails."""
     import importlib.util
     spec = importlib.util.spec_from_file_location("_ws_build", os.path.join(_HERE, "build.py"))
     mod = importlib.util.module_from_spec(spec)

@@ -1,7 +1,7 @@
-"""Builds libwebsplat_b200.so (sm_100a only) in-tree with nvcc.
+"""Builds libwebsplat_b200.so (sm_90a only, i.e. H100) in-tree with nvcc.
 
 Every translation unit is compiled with
-    -gencode arch=compute_100a,code=sm_100a -lineinfo -O3
+    -gencode arch=compute_90a,code=sm_90a -lineinfo -O3
 preprocess.cu additionally with -fmad=false (stage 1 is bit-exact against the CPU oracle:
 one IEEE rounding per written operation; the kernel is HBM-bound, so this costs nothing).
 """
@@ -16,7 +16,7 @@ OUT = os.path.join(HERE, "libwebsplat_b200.so")
 OBJ = os.path.join(HERE, "build")
 
 COMMON = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-Xptxas", "-v", "-Xptxas", "-warn-spills",
 ]
 UNITS = {
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
             if verbose:
                 sys.stderr.write(log)
     if jobs or force or _stale(OUT, objs):
-        cmd = [_nvcc(), "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+        cmd = [_nvcc(), "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         p = subprocess.run(cmd, capture_output=True, text=True)
         if p.returncode != 0:
             sys.stderr.write(p.stdout + p.stderr)

@@ -10,9 +10,9 @@
 // for the onesweep passes that follow.  The result after those passes is bit-identical
 // to sorting P 64-bit (tile|depth) keys with (tile, depth, slot) order, at ~1/3 of the traffic.
 //
-// Three launches, none with an inter-CTA dependency (a single-pass chained scan was measured
-// first, profiles/r01*: at ~900 pairs per partition every partition paid ~11 us of serialised
-// ticket / gather / look-back round trips and the kernel ran at 8 % of the HBM roofline):
+// Three launches, none with an inter-CTA dependency (a single-pass chained scan was tried
+// first: at ~900 pairs per partition every partition paid serialised ticket / gather /
+// look-back round trips and the kernel ran far below the HBM roofline):
 //   COUNT   pairs per 1024-splat partition (slot load + rectangle gather, 4 per thread in flight);
 //   SCAN    one CTA: exclusive scan of the partition totals, P, overflow flag;
 //   EXPAND  load-balanced over PAIRS, not splats: every splat with at least one tile drops a
@@ -22,11 +22,11 @@
 //           one multiply-high (magic reciprocal of the rectangle width).  Threads emit
 //           consecutive pairs straight to global memory, perfectly coalesced, however uneven
 //           the rectangles are (a screen-filling splat simply owns many consecutive positions).
-//           (A round-2 rewrite -- owner thread walks its rectangle, the block walks the large ones,
+//           (A rewrite -- owner thread walks its rectangle, the block walks the large ones,
 //           pairs staged in shared memory -- is kept as bin_expand_kernel / WS_BIN_EXPAND=2: it
-//           executes a quarter of the instructions and is 13 % slower, profiles/r02d_*.)
-// The digit histogram uses plain shared-memory atomicAdd (no return value): measured at
-// 118-135 G warp-ops/s on B200 whatever the address spread, 25x a MATCH.ANY-aggregated update
+//           executes a quarter of the instructions and is slower.)
+// The digit histogram uses plain shared-memory atomicAdd (no return value): its rate does not
+// depend on the address spread, and a MATCH.ANY-aggregated update is far slower
 // (profiles/microbench/rank_primitives.cu).
 #include "ws_device.cuh"
 #include "ws_kernels.h"
@@ -49,9 +49,8 @@ struct SplatRects { uint32_t slot[BIN_SPT], xy[BIN_SPT], w[BIN_SPT], h[BIN_SPT],
 // the split point is a multiple of 4 so that the 16-byte slot loads stay aligned
 __device__ __forceinline__ void slab_bounds(const BinningArgs &a, uint32_t V, uint32_t &lo, uint32_t &hi)
 {
-    // the nearest near_pct % of the depth-sorted splats form the near slab (0 = the default, a quarter).  Measured on B200
-    // (profiles/r02i_*, frames/s at cfg3 | cfg4): 15 %: 916 | 460, 20 %: 930 | 477, 25 %: 927 | 473, 35 %: 901 | 473,
-    // 50 % (round 1): 880 | 458, 65 %: 844 | 442 -- a smaller near slab sorts fewer pairs that the far slab's cull would
+    // the nearest near_pct % of the depth-sorted splats form the near slab (0 = the default, a quarter: a sweep over
+    // 15-65 % at cfg3 and cfg4 peaked at 20-25 % on the previous target GPU; not re-swept on H100) -- a smaller near slab sorts fewer pairs that the far slab's cull would
     // have dropped; below ~20 % too few tiles are saturated when the far slab is binned.
     const uint32_t near = a.near_pct ? (uint32_t)(((uint64_t)V * a.near_pct) / 100u) : (V >> 2);
     const uint32_t split = (V - near) & ~3u;
@@ -128,7 +127,7 @@ bin_count_kernel(BinningArgs a)
     slab_bounds(a, V, lo, hi);
     const uint32_t nparts = (hi - lo + BIN_PART - 1u) / BIN_PART;
     // The saturation test reads the "saturated" flag of every tile of every small rectangle: random byte gathers from
-    // global memory in round 1 (r02a: 43 us for the far half of cfg3, long_scoreboard 10 warps per issue).  The whole map is
+    // global memory would stall on long scoreboard for most of the far half of the frame.  The whole map is
     // 8160 tiles at 1080p, 32 400 at 4K: each CTA packs it into ONE BIT per tile in shared memory (1-4 KB), and a rectangle
     // row becomes two shared-memory words and a funnel shift.
     const uint8_t *done = a.tile_done;
@@ -190,14 +189,14 @@ bin_scan_kernel(BinningArgs a)
     }
 }
 
-// ---- (3'') EXPAND, round-2 rewrite (WS_BIN_EXPAND=2; NOT the default: measured slower, see launch_binning) -------------
-// ncu on the round-1 kernel (profiles/r02a: 139 lane-instructions per emitted pair, 1168 SASS
-// instructions, the marker / prefix-max machinery executed for every output position) showed the general
+// ---- (3'') EXPAND, rewrite (WS_BIN_EXPAND=2; NOT the default: slower, see launch_binning) --------------------------------
+// Profiling the default kernel (~140 lane-instructions per emitted pair, the marker / prefix-max machinery executed
+// for every output position) showed the general
 // load-balancing scheme costing 3x what the data needs: a splat touches 3.5 tiles on average, so the owner thread
 // simply walks its own rectangle.  Only rectangles above EXP_SMALL tiles (close-ups, gaussian_scaling > 1) are expanded
 // cooperatively by the whole block, one 256-wide stride per rectangle.  Pairs are staged in shared memory at their
 // block-local output position (scan of the per-splat counts), so the stores to global memory stay perfectly
-// coalesced and the output order -- splat (depth order), then row-major tile -- is exactly that of round 1.
+// coalesced and the output order -- splat (depth order), then row-major tile -- is exactly that of the default kernel.
 constexpr int EXP_CAP = 4096;                         // staged pairs per chunk (2 x 16 KB)
 constexpr uint32_t EXP_SMALL = 32;                    // rectangles up to this many tiles are walked by their owner thread
 constexpr int EXP_BIG = 512;                          // cooperative list entries per partition (beyond: owner thread walks)
@@ -456,9 +455,8 @@ cudaError_t launch_binning(const BinningArgs &a, int grid_count, int grid_expand
     ac.done_in_smem = done_bytes ? 1u : 0u;
     bin_count_kernel<<<grid_count, BIN_THREADS, done_bytes, stream>>>(ac);
     bin_scan_kernel<<<1, 1024, 0, stream>>>(a);
-    // default: the round-1 kernel (markers + prefix-max).  Measured on B200 (profiles/r02d_*): 80.0 vs 90.7 us for the near
-    // slab of cfg3, binning 0.309 vs 0.399 ms at cfg4 -- the round-2 rewrite executes a quarter of the instructions but its
-    // owner-thread loops serialise on the longest rectangle of each warp and its scattered staging stores conflict.
+    // default: the markers + prefix-max kernel.  The rewrite executes a quarter of the instructions but is slower at cfg3
+    // and cfg4: its owner-thread loops serialise on the longest rectangle of each warp and its scattered staging stores conflict.
     static const int variant = [] { const char *e = getenv("WS_BIN_EXPAND"); return (e && atoi(e) == 2) ? 2 : 1; }();
     if (variant == 1) bin_expand_v1_kernel<<<grid_expand, BIN_THREADS, 0, stream>>>(a);
     else bin_expand_kernel<<<grid_expand, BIN_THREADS, 0, stream>>>(a);

@@ -64,7 +64,7 @@ extern "C" const char *ws_status_string(ws_status s)
     }
 }
 extern "C" const char *ws_last_error(void) { return g_last_error.c_str(); }
-extern "C" const char *ws_version(void) { return "websplat_b200 0.1 (sm_100a)"; }
+extern "C" const char *ws_version(void) { return "websplat_b200 0.1 (sm_90a)"; }
 
 // ------------------------------------------------------------------------------------
 struct ws_context {
@@ -84,7 +84,7 @@ extern "C" ws_status ws_context_create(int cuda_device, ws_context **out)
     if (cuda_device < 0 || cuda_device >= count) return fail(WS_ERR_INVALID_ARGUMENT, "cuda_device out of range");
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, cuda_device));
-    if (prop.major != 10) return fail(WS_ERR_CUDA, "device is not compute capability 10.x (library is built for sm_100a only)");
+    if (prop.major != 9 || prop.minor != 0) return fail(WS_ERR_CUDA, "device is not compute capability 9.0 (library is built for sm_90a only)");
     CU(cudaSetDevice(cuda_device));
     ws_context *c = new (std::nothrow) ws_context();
     if (!c) return fail(WS_ERR_OUT_OF_MEMORY, "host allocation failed");
@@ -820,7 +820,7 @@ extern "C" ws_status ws_renderer_create(ws_context *ctx, ws_format fmt, uint32_t
     r->grid_pre = ctx->sm_count * preprocess_blocks_per_sm(r->compressed);
     r->grid_sort = ctx->sm_count * sort_pass_blocks_per_sm();
     r->grid_bin = ctx->sm_count * binning_blocks_per_sm();
-    {   // A/B knobs (profiles/): fewer resident CTAs per SM for the persistent kernels leave room for the other frame's kernels
+    {   // A/B knobs: fewer resident CTAs per SM for the persistent kernels leave room for the other frame's kernels
         auto per_sm = [&](const char *name, int cur) { const char *e = getenv(name); const int k = e ? atoi(e) : 0; return (k >= 1 && k * ctx->sm_count < cur) ? k * ctx->sm_count : cur; };
         r->grid_pre = per_sm("WS_PRE_CTAS_PER_SM", r->grid_pre);
         r->grid_sort = per_sm("WS_SORT_CTAS_PER_SM", r->grid_sort);
@@ -873,7 +873,7 @@ static uint32_t split_near_pct()
     return v;
 }
 
-// compositor: cull against the box of still-unsaturated pixels (WS_ACTIVE_CULL=0 turns it off for A/B runs in profiles/)
+// compositor: cull against the box of still-unsaturated pixels (WS_ACTIVE_CULL=0 turns it off for A/B runs)
 static int active_cull_default()
 {
     static const int v = [] { const char *e = getenv("WS_ACTIVE_CULL"); return (e && atoi(e) == 0) ? 0 : 1; }();
@@ -994,8 +994,8 @@ static ws_status validate_frame(ws_renderer *r, ws_pointcloud *pc, const ws_spla
 }
 
 // Occlusion split on/off for this frame + the per-pixel state buffer it needs.  `points_here` = Gaussians this GPU
-// depth-sorts (the whole cloud; total / world for sharded frames).  Automatic threshold: measured on one GPU cfg1
-// (100 K points) -14 %, cfg2 (1 M) -2 %, cfg3 (6 M) +7 % -- the six extra launches and the state round trip pay off only
+// depth-sorts (the whole cloud; total / world for sharded frames).  Automatic threshold (2 M points), chosen on the
+// previous target GPU and not re-measured on H100: the split slowed cfg1 (100 K points) and cfg2 (1 M) and sped up cfg3 (6 M) -- the six extra launches and the state round trip pay off only
 // when there are many pairs to save.
 static ws_status decide_split(ws_renderer *r, uint64_t points_here, uint32_t W, uint32_t H)
 {
@@ -1487,8 +1487,8 @@ extern "C" ws_status ws_renderer_shard_frame_to_root(ws_renderer *r, ws_pointclo
     };
 
     if (r->use_graphs && !r->timing) {
-        // One CUDA graph per frame-buffer parity: ~25 launches + 3 clears become one launch (host: ~200 -> ~60 us per
-        // frame and rank; device: no launch gaps between the latency-bound kernels of a 1/8 share of the frame).
+        // One CUDA graph per frame-buffer parity: ~25 launches + 3 clears become one launch (host: a third of the
+        // launch cost per frame and rank; device: no launch gaps between the latency-bound kernels of a 1/8 share of the frame).
         auto &k = s.frame_key[par];
         bool same = s.frame_exec[par] && k.pc_gen == pc->generation && k.buf_gen == r->buf_generation && k.root == root &&
                     k.gated == s.gated && k.split == r->frame_split;

@@ -1,4 +1,4 @@
-// composite.cu -- stage 3: tile-binned front-to-back alpha compositing on sm_100a.
+// composite.cu -- stage 3: tile-binned front-to-back alpha compositing on sm_90a.
 //
 // Replaces the reference's instanced-quad draw + fixed-function blending: vs_main/fs_main
 // (gaussian.wgsl:30-66) and PREMULTIPLIED_ALPHA_BLENDING (renderer.rs:63-67).  Per pixel the
@@ -18,8 +18,8 @@
 //  * the centre is expressed relative to the tile origin with exact f16 x integer products,
 //    so `a` carries ~1e-5 absolute error at 4K instead of ulp(3840);
 //  * the per-hit code is branch-free and keeps no `done` flag: a pixel whose transmittance falls below 2^-16 has its
-//    T set to exactly 0, after which every further weight is exactly 0 (round 1 tested a flag per hit: 35 SASS
-//    instructions per warp x splat hit, 28 now -- the kernel is issue-bound, profiles/r02*_ncu_summary.md).
+//    T set to exactly 0, after which every further weight is exactly 0 (a flag tested per hit cost 7 more SASS
+//    instructions per warp x splat hit -- the kernel is issue-bound).
 #include "ws_device.cuh"
 #include "ws_kernels.h"
 

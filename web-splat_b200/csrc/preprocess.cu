@@ -1,25 +1,25 @@
-// preprocess.cu -- stage 1 of the splat render path on sm_100a.
+// preprocess.cu -- stage 1 of the splat render path on sm_90a.
 //
 // Replaces preprocess.wgsl:163-280 / preprocess_compressed.wgsl:206-331 of the reference
 // (one thread per Gaussian: cull, 3D->2D covariance, eigen axes, SH colour, f16 pack,
 // depth key) and adds what the tile-binned design needs: the per-splat 16x16-tile
 // rectangle and the digit histograms of the depth keys for the onesweep that follows.
 //
-// B200 design notes
+// Design notes
 //  * three launches: (1) COUNT reads only a 12-B xyz plane, culls, writes the number of
 //    survivors of every 256-Gaussian partition and the digit histograms of their depth keys;
 //    (2) a one-CTA SCAN turns the counts into slot offsets; (3) MAIN does the projection.
 //    Compaction is therefore deterministic (slot order = Gaussian index order; the reference
 //    uses one contended global atomic, preprocess.wgsl:262, whose order is not), and MAIN has
-//    no inter-CTA dependency at all -- a single-pass chained scan was tried first (r01a/r01b in
-//    profiles/): its look-back serialised the prefetch pipeline.  The price is re-reading xyz:
+//    no inter-CTA dependency at all -- a single-pass chained scan was tried first: its
+//    look-back serialised the prefetch pipeline.  The price is re-reading xyz:
 //    +12 B on top of 124 B per Gaussian;
 //  * MAIN is software-pipelined: partitions are assigned round-robin, the 28-B (24-B) AoS
 //    records of partition k+1 and -- when at least half of it survives -- its 24-KB SH block
 //    are fetched by cp.async.bulk (TMA engine, UBLKCP) into shared-memory rings while
-//    partition k is being computed; 3 CTAs x 31 KB per SM are in flight, HBM sees only full bursts;
-//    sparse partitions fetch SH with three 256-bit loads per surviving lane instead
-//    (one full 32-B sector per request);
+//    partition k is being computed; 3 CTAs per SM are in flight, HBM sees only full bursts;
+//    sparse partitions fetch SH with three 32-B sectors per surviving lane instead
+//    (two adjacent 128-bit loads each, so every sector is fetched whole);
 //  * records are read from shared memory at a conflict-free 7-word (6-word: 2-way) stride;
 //    outputs are staged through shared memory and leave as coalesced streams;
 //  * this file is compiled with -fmad=false, so a fused multiply-add happens exactly where fmaf() is
@@ -147,11 +147,13 @@ __device__ __forceinline__ V3 evaluate_sh(float x, float y, float z, const SH &s
     return result;
 }
 
-__device__ __forceinline__ void ldg256(const void *p, uint32_t *r)
+// one 32-B sector as two 128-bit loads (sm_90 has no 256-bit load); both halves are issued before either is used
+__device__ __forceinline__ void ldg_sector(const void *p, uint32_t *r)
 {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "l"(p));
+    asm volatile("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+    asm volatile("ld.global.nc.L1::no_allocate.v4.b32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "l"((const uint8_t *)p + 16));
 }
 
 struct Stage1 {
@@ -354,7 +356,7 @@ count_kernel(PreprocessArgs a)
     constexpr int NDIG = 4;
     // CNT_UNROLL consecutive partitions per trip: their 3 * CNT_UNROLL loads are issued before the first use, and the
     // block-wide counts (one barrier each) follow back to back -- a single partition per trip left the loads exposed
-    // behind every barrier (r01m: long_scoreboard 35 %, 1.9 TB/s)
+    // behind every barrier (long-scoreboard stalls dominated)
     constexpr uint32_t CNT_UNROLL = 4;
     for (uint32_t part0 = blockIdx.x * CNT_UNROLL; part0 < nparts; part0 += gridDim.x * CNT_UNROLL) {
         float px[CNT_UNROLL], py[CNT_UNROLL], pz[CNT_UNROLL];
@@ -379,8 +381,8 @@ count_kernel(PreprocessArgs a)
             const uint32_t cnt = (uint32_t)__syncthreads_count(keep[u] ? 1 : 0);
             if (tid == 0 && part0 + u < nparts) a.part_counts[part0 + u] = cnt;
         }
-        // shared atomics without return sustain ~120 G warp-ops/s on B200 whatever the spread
-        // (profiles/microbench/rank_primitives.cu); MATCH-aggregating them was 25x slower
+        // shared atomics without return keep their rate whatever the spread
+        // (profiles/microbench/rank_primitives.cu); MATCH-aggregating them is far slower
 #pragma unroll
         for (uint32_t u = 0; u < CNT_UNROLL; u++) {
             if (keep[u]) {
@@ -521,12 +523,12 @@ preprocess_kernel(PreprocessArgs a)
                         }
                     } else {
                         const uint8_t *sp = a.sh_coefs + (size_t)idx * 96u;
-                        ldg256(sp, sh.w);
-                        if (deg > 1u) ldg256(sp + 32, sh.w + 8); else {
+                        ldg_sector(sp, sh.w);
+                        if (deg > 1u) ldg_sector(sp + 32, sh.w + 8); else {
 #pragma unroll
                             for (int i = 8; i < 16; i++) sh.w[i] = 0u;
                         }
-                        if (deg > 2u) ldg256(sp + 64, sh.w + 16); else {
+                        if (deg > 2u) ldg_sector(sp + 64, sh.w + 16); else {
 #pragma unroll
                             for (int i = 16; i < 24; i++) sh.w[i] = 0u;
                         }

@@ -1,4 +1,4 @@
-// radix_sort.cu -- stage 2: onesweep LSD radix sort of (u32 key, u32 value) pairs on sm_100a.
+// radix_sort.cu -- stage 2: onesweep LSD radix sort of (u32 key, u32 value) pairs on sm_90a.
 //
 // Replaces the reference's Fuchsia-derived WGSL sort (radix_sort.wgsl:48-512, driven by
 // gpu_rs.rs:764-863): same contract -- stable, ascending, 8-bit digits, result back in the
@@ -8,11 +8,10 @@
 //     which radix_sort.wgsl:365-387 silently relies on);
 //   * ranking: each lane ORs its lane bit into a per-warp, per-digit peer mask in shared memory
 //     (atomicOr without return), reads the mask back and the lowest peer bumps the warp's
-//     private digit counter with a plain read-modify-write.  Measured on B200
-//     (profiles/microbench/rank_primitives.cu): MATCH.ANY on random 8-bit digits sustains only
-//     4.7 G warp-ops/s chip-wide (its cost grows with the number of distinct values), an
-//     8-ballot emulation 11.5 G, shared atomics without return 118-135 G; the reference
-//     emulates match with a per-key shared-memory loop (radix_sort.wgsl:283-302);
+//     private digit counter with a plain read-modify-write.  MATCH.ANY on random 8-bit digits
+//     costs more the more distinct values a warp holds, and an 8-ballot emulation is also slower
+//     than shared atomics without return (profiles/microbench/rank_primitives.cu compares the
+//     three); the reference emulates match with a per-key shared-memory loop (radix_sort.wgsl:283-302);
 //   * decoupled look-back, one thread per digit bin, on single 32-bit status words
 //     (2-bit flag | 30-bit count: relaxed accesses suffice), TWO levels deep: partitions are
 //     grouped by 16 and the last partition of a group publishes the group's aggregate /
@@ -35,7 +34,7 @@ namespace {
 
 constexpr int WARPS = SORT_THREADS / 32;
 #ifndef WS_RANK_WAYS
-#define WS_RANK_WAYS 1                         // items ranked per step; 1, 2 and 4 are built (WS_RANK_WAYS env). Measured cfg3 tile pass: 0.135 | 0.137 | 0.141 ms -- the pass is bound by shared-memory wavefronts (bank conflicts on random digits), not by the dependent chain
+#define WS_RANK_WAYS 1                         // items ranked per step; 1, 2 and 4 are built (WS_RANK_WAYS env). 1 was fastest on the cfg3 tile pass -- the pass is bound by shared-memory wavefronts (bank conflicts on random digits), not by the dependent chain
 #endif
 struct LbState { uint32_t excl; bool done; };
 
@@ -43,10 +42,9 @@ struct LbState { uint32_t excl; bool done; };
 // `col` already points at this thread's bin column.  Up to LB_WIDTH relaxed loads are issued per
 // step (they are independent), then consumed in order; an unpublished word restarts the step at
 // that row.  Rows below lo end the level; when `below_is_prefix` they count as "inclusive prefix 0".
-// LB_WIDTH: round 1 issued 4 loads per step; ncu (profiles/r02a: 37 % of the pass's executed warp
-// instructions and 25 % of its stall samples sit in this loop) showed the walk over up to 15 + W/16
-// rows -- a persistent grid starts W = 444 partitions at once, none with a prefix -- costing ~8
-// dependent L2 round trips per partition; 16 loads per step make it ~3.
+// LB_WIDTH: with 4 loads per step a large share of the pass's instructions and stalls sat in this loop:
+// the walk over up to 15 + W/16 rows -- a persistent grid starts W partitions at once (W = 396 on
+// 132 SMs), none with a prefix -- cost ~8 dependent L2 round trips per partition; 16 loads per step make it ~3.
 #ifndef WS_LB_WIDTH
 #define WS_LB_WIDTH 16
 #endif
@@ -76,10 +74,12 @@ __device__ __forceinline__ void lookback_level(const uint32_t *col, int p, int l
 }
 
 #ifndef WS_SORT_CTAS
-#define WS_SORT_CTAS 3                         // resident CTAs per SM the pass is compiled for (4 = 64 registers: A/B knob, profiles/microbench)
+// resident CTAs per SM the pass is compiled for (A/B knob).  On sm_90a, 3 caps the pass at 80 registers and it spills;
+// 2 (122 registers, no spill) sorts 15-20 % faster on H100 (profiles/microbench: sort_vs_cub vs sort_vs_cub_c3, every shape), 4 is slower still
+#define WS_SORT_CTAS 2
 #endif
 template <bool EMIT_RANGES, int RANK_WAYS>
-__global__ void __launch_bounds__(SORT_THREADS, WS_SORT_CTAS)   // round 1: 16 items x 3 CTAs/SM measured best: 8 items x 4 CTAs and 16 items x 4 CTAs (spilling) were 7-10 % slower
+__global__ void __launch_bounds__(SORT_THREADS, WS_SORT_CTAS)   // 16 items per thread
 onesweep_pass_kernel(SortPassArgs a)
 {
     __shared__ __align__(16) uint32_t s_keys[SORT_PART];      // during ranking s_keys / s_vals double as the peer masks
@@ -318,8 +318,8 @@ onesweep_pass_kernel(SortPassArgs a)
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// V2 of the pass (WS_SORT_VARIANT=2; NOT the default -- measured, profiles/r02a_*): what ncu named on V1 (r01m/r01q: SM 30-37 %, short_scoreboard 28-33 % + long_scoreboard
-// 20-25 %, ~38 shared-memory wavefront cycles per warp-item on random digits) is attacked three ways:
+// V2 of the pass (WS_SORT_VARIANT=2; NOT the default): what profiling named on V1 (short and long scoreboard stalls,
+// many shared-memory wavefront cycles per warp-item on random digits) is attacked three ways:
 //   * TMA staging: the NEXT partition's keys and values (2 x 16 KB) are fetched by cp.async.bulk (UBLKCP) into a
 //     staging buffer while the current partition is in its look-back and write-out; the ticket of the next partition
 //     is taken at the top of the iteration, so neither the ticket round trip nor the two global-load latencies sit
@@ -331,11 +331,10 @@ onesweep_pass_kernel(SortPassArgs a)
 // Also: a pass whose digit is the same for every key (one histogram bin holds all n keys -- the top byte of the
 // compressed layout's 24-bit key) degenerates to a plain copy, and the last tile pass may skip the key store
 // (keys_out == NULL: the compositor only needs the values and the tile ranges).
-// RESULT (B200, profiles/r02a_sort_v{1,2}.jsonl): no faster than V1 on its own (depth pass 49.9 vs 48.9 us, 21 M-pair tile
-// pass 138.7 vs 133.6 us, 10.5 M pairs 71.2 vs 73.2 us) -- neither the load latency nor the shared-memory wavefronts were
-// the bound; the look-back walk was (see lookback_level) -- and with two frames in flight the frame rate FELL from 819
-// to 237 frames/s: 3 CTAs x 75 KB take every SM's shared memory, so no kernel of the other frame can ever share an SM
-// with a sort pass.  V1 (41 KB static) stays the default; V2 is kept as the measured TMA-staged alternative.
+// RESULT: no faster than V1 on its own -- neither the load latency nor the shared-memory wavefronts were the bound; the
+// look-back walk was (see lookback_level) -- and with two frames in flight the frame rate fell to a fraction: 3 CTAs x
+// 75 KB take nearly all of an SM's 228 KB of shared memory, so no kernel of the other frame can ever share an SM with a
+// sort pass.  V1 (41 KB static) stays the default; V2 is kept as the TMA-staged alternative.
 struct SortSmemV2 {
     uint32_t stage_k[SORT_PART];              // TMA destination: next partition's keys ...
     uint32_t stage_v[SORT_PART];              // ... and values
@@ -560,7 +559,7 @@ sort_histogram_kernel(const uint32_t *__restrict__ keys, const uint32_t *n_ptr, 
     if (n > n_cap) n = n_cap;
     for (uint32_t i = blockIdx.x * 256u + tid; i < n; i += gridDim.x * 256u) {
         const uint32_t k = keys[i];
-        for (int d = 0; d < passes; d++) atomicAdd(&s_hist[d * 256 + ((k >> (8 * d)) & 255u)], 1u);   // shared atomics w/o return: ~120 G warp-ops/s
+        for (int d = 0; d < passes; d++) atomicAdd(&s_hist[d * 256 + ((k >> (8 * d)) & 255u)], 1u);   // shared atomics without return
     }
     __syncthreads();
     for (unsigned i = tid; i < (unsigned)passes * 256u; i += 256u) {
@@ -574,7 +573,7 @@ sort_histogram_kernel(const uint32_t *__restrict__ keys, const uint32_t *n_ptr, 
 static int rank_ways()
 {
     static int ways = [] {
-        const char *e = getenv("WS_RANK_WAYS");              // tuning knob for profiles/; the default is what ships
+        const char *e = getenv("WS_RANK_WAYS");              // tuning knob for A/B runs; the default is what ships
         const int w = e ? atoi(e) : WS_RANK_WAYS;
         return (w == 1 || w == 2 || w == 4) ? w : WS_RANK_WAYS;
     }();
@@ -584,7 +583,7 @@ static int rank_ways()
 static int sort_variant()
 {
     static int v = [] {
-        const char *e = getenv("WS_SORT_VARIANT");           // 1 = register-staged pass (default), 2 = the TMA-staged pass (measured alternative, see above)
+        const char *e = getenv("WS_SORT_VARIANT");           // 1 = register-staged pass (default), 2 = the TMA-staged pass (alternative, see above)
         const int w = e ? atoi(e) : 1;
         return (w == 2) ? 2 : 1;
     }();

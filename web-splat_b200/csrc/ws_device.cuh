@@ -1,4 +1,4 @@
-// ws_device.cuh -- shared device-side definitions for the sm_100a splat render path.
+// ws_device.cuh -- shared device-side definitions for the sm_90a splat render path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -179,7 +179,7 @@ __device__ __forceinline__ bool wait_epoch(const uint32_t *flag, uint32_t epoch,
 // Exclusive scan of counts[0..n) into bases[0..n) by ONE CTA of 1024 threads; returns the total (64-bit) to every thread.
 // 16 K-element tiles, sixteen adjacent elements per thread (four 128-bit loads in flight before the first use): every
 // element is read once, scanned in registers + shuffles, written once; three barriers per tile.  cfg3's 23.4 K partition
-// counts are two tiles (the round-1 version used 4 K tiles: six dependent trips, 14 us).  The running total is kept in
+// counts are two tiles (4 K tiles would take six dependent trips).  The running total is kept in
 // 64 bits: pair counts can exceed 2^32 (screen-filling splats); bases saturate at 0xffffffff, which every consumer
 // treats as "beyond capacity", so an overflow is reported instead of wrapping into a silently wrong frame.
 // counts / bases must be 16-byte aligned (they are 256-byte aligned slices of the scratch allocation).

@@ -1,4 +1,4 @@
-// ws_kernels.h -- host-visible launchers of the sm_100a kernels (internal to the library).
+// ws_kernels.h -- host-visible launchers of the sm_90a kernels (internal to the library).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
