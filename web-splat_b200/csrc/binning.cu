@@ -87,9 +87,8 @@ __device__ __forceinline__ void load_rects(const BinningArgs &a, uint32_t first,
 // Returns the keep bytes for load_rects (the expand kernel does not repeat the test, nor fetch the dropped rectangles).
 // `done` is the per-tile byte map (global memory, or its copy in shared memory); `bits`, when not NULL, is the same map as
 // one BIT per tile in shared memory: a row of up to 16 tiles is then one funnel-shifted compare instead of a byte per tile.
-__device__ __forceinline__ uint32_t drop_saturated(const BinningArgs &a, SplatRects &r, const uint8_t *done, const uint32_t *bits)
+__device__ __forceinline__ uint32_t drop_saturated(uint32_t tiles_x, SplatRects &r, const uint8_t *done, const uint32_t *bits)
 {
-    const uint32_t tiles_x = a.uniforms->tiles_x;
     uint32_t keep4 = 0u;
 #pragma unroll
     for (int j = 0; j < BIN_SPT; j++) {
@@ -115,49 +114,60 @@ __device__ __forceinline__ uint32_t drop_saturated(const BinningArgs &a, SplatRe
     return keep4;
 }
 
+// The saturation test reads the "saturated" flag of every tile of every small rectangle: random byte gathers from
+// global memory would stall on long scoreboard for most of the far half of the frame.  The whole map is
+// 8160 tiles at 1080p, 32 400 at 4K: each CTA packs it into ONE BIT per tile in shared memory (1-4 KB), and a rectangle
+// row becomes two shared-memory words and a funnel shift.  Called by the whole CTA; ends with a barrier.
+__device__ __forceinline__ void pack_done_bits(const uint8_t *tile_done, uint32_t T, uint32_t *s_bits)
+{
+    const uint32_t nwords = (T + 31u) / 32u;
+    for (uint32_t w = threadIdx.x; w <= nwords; w += blockDim.x) {     // one word past the end stays 0: the funnel shift reads w0 + 1
+        uint32_t v = 0u;
+        if (w < nwords) {
+            const uint4 *src = reinterpret_cast<const uint4 *>(tile_done + (size_t)w * 32u);   // 32 flag bytes (allocation padded)
+            const uint4 q0 = src[0], q1 = src[1];
+            const uint32_t b[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+#pragma unroll
+            for (int k = 0; k < 8; k++) {                              // byte i of the 32 -> bit i (flags are 0 / 1)
+                v |= ((b[k] & 0x1u) | ((b[k] >> 7) & 0x2u) | ((b[k] >> 14) & 0x4u) | ((b[k] >> 21) & 0x8u)) << (4 * k);
+            }
+            const uint32_t valid = T - w * 32u;                         // tiles beyond T (padding bytes) never count as done... nor matter
+            if (valid < 32u) v &= (1u << valid) - 1u;
+        }
+        s_bits[w] = v;
+    }
+    __syncthreads();
+}
+
+// bytes of dynamic shared memory for the bit map (0: too many tiles, the test reads the byte map from global memory).
+// One bit per tile + one spare word; up to 16384 x 16384 pixels = 1 Mi tiles = 128 KB would not fit the default 48 KB:
+// above 256 Ki tiles the kernels read the byte map from global memory.
+static size_t done_bits_bytes(uint32_t num_tiles)
+{
+    return (num_tiles && num_tiles <= 262144u) ? (((size_t)num_tiles + 31u) / 32u + 1u) * 4u : 0u;
+}
+
 // ---- (1) COUNT ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(BIN_THREADS)
 bin_count_kernel(BinningArgs a)
 {
     __shared__ uint32_t s_red[BIN_WARPS];
-    extern __shared__ __align__(16) uint8_t s_done[];   // far slab: the per-tile "saturated" bytes (T of them, when they fit)
+    extern __shared__ __align__(16) uint8_t s_done[];   // far slab: the per-tile "saturated" map, one bit per tile (when it fits)
     const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    const uint32_t V = a.counters->num_visible;
+    const uint32_t V = *a.list_len;
     uint32_t lo, hi;
     slab_bounds(a, V, lo, hi);
     const uint32_t nparts = (hi - lo + BIN_PART - 1u) / BIN_PART;
-    // The saturation test reads the "saturated" flag of every tile of every small rectangle: random byte gathers from
-    // global memory would stall on long scoreboard for most of the far half of the frame.  The whole map is
-    // 8160 tiles at 1080p, 32 400 at 4K: each CTA packs it into ONE BIT per tile in shared memory (1-4 KB), and a rectangle
-    // row becomes two shared-memory words and a funnel shift.
     const uint8_t *done = a.tile_done;
     const uint32_t *bits = nullptr;
     if (a.tile_done && a.done_in_smem) {
-        uint32_t *s_bits = reinterpret_cast<uint32_t *>(s_done);
-        const uint32_t T = a.uniforms->tiles_x * a.uniforms->tiles_y;
-        const uint32_t nwords = (T + 31u) / 32u;
-        for (uint32_t w = tid; w <= nwords; w += BIN_THREADS) {         // one word past the end stays 0: the funnel shift reads w0 + 1
-            uint32_t v = 0u;
-            if (w < nwords) {
-                const uint4 *src = reinterpret_cast<const uint4 *>(a.tile_done + (size_t)w * 32u);   // 32 flag bytes (allocation padded)
-                const uint4 q0 = src[0], q1 = src[1];
-                const uint32_t b[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-#pragma unroll
-                for (int k = 0; k < 8; k++) {                          // byte i of the 32 -> bit i (flags are 0 / 1)
-                    v |= ((b[k] & 0x1u) | ((b[k] >> 7) & 0x2u) | ((b[k] >> 14) & 0x4u) | ((b[k] >> 21) & 0x8u)) << (4 * k);
-                }
-                const uint32_t valid = T - w * 32u;                     // tiles beyond T (padding bytes) never count as done... nor matter
-                if (valid < 32u) v &= (1u << valid) - 1u;
-            }
-            s_bits[w] = v;
-        }
-        __syncthreads();
-        bits = s_bits;
+        pack_done_bits(a.tile_done, a.uniforms->tiles_x * a.uniforms->tiles_y, reinterpret_cast<uint32_t *>(s_done));
+        bits = reinterpret_cast<const uint32_t *>(s_done);
     }
     for (uint32_t part = blockIdx.x; part < nparts; part += gridDim.x) {
         SplatRects r;
         load_rects(a, lo + part * BIN_PART + tid * BIN_SPT, hi, r);
-        if (a.tile_done) a.keep4[part * BIN_THREADS + tid] = drop_saturated(a, r, done, bits);
+        if (a.tile_done) a.keep4[part * BIN_THREADS + tid] = drop_saturated(a.uniforms->tiles_x, r, done, bits);
         uint32_t c = r.cnt[0] + r.cnt[1] + r.cnt[2] + r.cnt[3];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
@@ -177,7 +187,7 @@ bin_count_kernel(BinningArgs a)
 __global__ void __launch_bounds__(1024)
 bin_scan_kernel(BinningArgs a)
 {
-    const uint32_t V = a.counters->num_visible;
+    const uint32_t V = *a.list_len;
     uint32_t lo, hi;
     slab_bounds(a, V, lo, hi);
     const uint32_t nparts = (hi - lo + BIN_PART - 1u) / BIN_PART;
@@ -212,7 +222,7 @@ bin_expand_kernel(BinningArgs a)
     __shared__ uint32_t s_nbig;
 
     const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    const uint32_t V = a.counters->num_visible;
+    const uint32_t V = *a.list_len;
     uint32_t lo, hi;
     slab_bounds(a, V, lo, hi);
     const uint32_t nparts = (hi - lo + BIN_PART - 1u) / BIN_PART;
@@ -318,7 +328,9 @@ bin_expand_kernel(BinningArgs a)
 constexpr int BIN_ROUNDS = 8;                         // (v1) output positions per thread and chunk
 constexpr int BIN_CAP = BIN_THREADS * BIN_ROUNDS;     // (v1) 2048 pairs per chunk
 // ---- (3) EXPAND (default): load-balanced over PAIRS with markers + prefix-max -----------------------------------------
-__global__ void __launch_bounds__(BIN_THREADS, 4)
+// (5 resident CTAs per SM: the binning grid is sized by this kernel's occupancy; at 4 the register allocation may grow
+// past 48 and the persistent grid of both binning kernels shrinks by a fifth)
+__global__ void __launch_bounds__(BIN_THREADS, 5)
 bin_expand_v1_kernel(BinningArgs a)
 {
     __shared__ uint32_t s_owner[BIN_CAP];             // marker = owner index + 1 at the owner's first position
@@ -329,7 +341,7 @@ bin_expand_v1_kernel(BinningArgs a)
     __shared__ uint32_t s_wcarry[BIN_WARPS];
 
     const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    const uint32_t V = a.counters->num_visible;
+    const uint32_t V = *a.list_len;
     uint32_t lo, hi;
     slab_bounds(a, V, lo, hi);
     const uint32_t nparts = (hi - lo + BIN_PART - 1u) / BIN_PART;
@@ -443,15 +455,259 @@ bin_expand_v1_kernel(BinningArgs a)
     }
 }
 
+// ---- occlusion split on one GPU ------------------------------------------------------------------------------------
+// The near slab does not need a global depth order to be chosen: a key VALUE does as well as a position (the image is
+// the same wherever the cut is, DESIGN.md section 4), and the far slab's cull is a per-splat test against the saturated
+// tiles.  So: pick the cut from a histogram of the keys, compact the near list (key >= cut) and depth-sort only it;
+// after its composite, cull the far splats in slot order and depth-sort only the survivors.  Equal keys fall on the
+// same side of the cut, and both lists are compacted in slot order, so the stable sort of each list is the order the
+// full sort gives them.
+static_assert(SPLIT_CUT_BINS == BIN_THREADS * 8, "the cut is picked by one CTA, eight bins per thread");
+
+// the BIN_SPT consecutive keys first .. first+3 (0 beyond V)
+__device__ __forceinline__ void load_keys4(const uint32_t *keys, uint32_t first, uint32_t V, uint32_t k[BIN_SPT])
+{
+    if (first + BIN_SPT <= V) {
+        const uint4 q = *reinterpret_cast<const uint4 *>(keys + first);
+        k[0] = q.x; k[1] = q.y; k[2] = q.z; k[3] = q.w;
+    } else {
+#pragma unroll
+        for (int j = 0; j < BIN_SPT; j++) k[j] = (first + j < V) ? keys[first + j] : 0u;
+    }
+}
+
+// inclusive scan of one value per thread over the CTA (BIN_THREADS threads); s_w: BIN_WARPS words
+__device__ __forceinline__ uint32_t block_inclusive_scan(uint32_t v, uint32_t *s_w)
+{
+    const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, v, o);
+        if ((int)lane >= o) v += t;
+    }
+    if (lane == 31) s_w[warp] = v;
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < BIN_WARPS; k++) if (k < (int)warp) v += s_w[k];
+    return v;
+}
+
+// Histogram of (key - kmin) >> s over the V keys, s the smallest shift that leaves at most SPLIT_CUT_BINS bins; the last
+// CTA to finish walks it from the nearest bin down and sets the cut at the boundary of the bin where the count reaches
+// the near slab's share (at least one splat when V > 0).  A cut at a bin boundary never separates equal keys.
+__global__ void __launch_bounds__(BIN_THREADS)
+split_cut_kernel(SplitArgs a)
+{
+    __shared__ uint32_t s_hist[SPLIT_CUT_BINS];
+    __shared__ uint32_t s_w[BIN_WARPS];
+    __shared__ bool s_last;
+    const unsigned tid = threadIdx.x;
+    const uint32_t V = a.counters->num_visible;
+    const uint32_t kmin = ~a.counters->key_min_inv, span = a.counters->key_max - kmin;
+    uint32_t s = 0;
+    while ((span >> s) >= (uint32_t)SPLIT_CUT_BINS) s++;
+    for (unsigned i = tid; i < (unsigned)SPLIT_CUT_BINS; i += BIN_THREADS) s_hist[i] = 0u;
+    __syncthreads();
+    // a small grid (every CTA flushes up to 2048 bins into global memory at the end) with CUT_UNROLL 16-B loads per
+    // thread in flight, so that the sweep still keeps enough bytes in flight to stream the keys at DRAM rate
+    constexpr uint32_t CUT_UNROLL = 4, STEP = BIN_THREADS * BIN_SPT;
+    for (uint32_t first0 = blockIdx.x * STEP * CUT_UNROLL + tid * BIN_SPT; first0 < V; first0 += gridDim.x * STEP * CUT_UNROLL) {
+        uint32_t k[CUT_UNROLL][BIN_SPT];
+#pragma unroll
+        for (uint32_t u = 0; u < CUT_UNROLL; u++) load_keys4(a.keys, first0 + u * STEP, V, k[u]);
+#pragma unroll
+        for (uint32_t u = 0; u < CUT_UNROLL; u++)
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) if (first0 + u * STEP + j < V) atomicAdd(&s_hist[(k[u][j] - kmin) >> s], 1u);
+    }
+    __syncthreads();
+    for (unsigned i = tid; i < (unsigned)SPLIT_CUT_BINS; i += BIN_THREADS) {
+        const uint32_t c = s_hist[i];
+        if (c) atomicAdd(a.cut_hist + i, c);
+    }
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(&a.counters->cut_done, 1u) == gridDim.x - 1u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    uint32_t target = a.near_pct ? (uint32_t)(((uint64_t)V * a.near_pct) / 100u) : (V >> 2);
+    if (target == 0u) target = V ? 1u : 0u;
+    const int top = SPLIT_CUT_BINS - 1 - 8 * (int)tid;                 // thread 0 owns the nearest 8 bins
+    uint32_t c8[8], sum = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) { c8[k] = __ldcg(a.cut_hist + top - k); sum += c8[k]; }
+    const uint32_t incl = block_inclusive_scan(sum, s_w);
+    const uint32_t excl = incl - sum;
+    if (target > 0u && excl < target && target <= incl) {               // exactly one thread: the counts sum to V >= target
+        uint32_t acc = excl;
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            acc += c8[k];
+            if (acc >= target) { a.counters->split_cut = kmin + ((uint32_t)(top - k) << s); break; }
+        }
+    }
+}
+
+// COUNT: which splats of every 1024-splat partition (slot order) enter the list.  Near: key >= cut.  Far: key < cut, a
+// non-empty rectangle, and not all of its tiles saturated (drop_saturated, the rule of the position-split far slab).
+// The decisions leave as one ballot word per (warp, splat of the thread): 32 words per partition.
+__global__ void __launch_bounds__(BIN_THREADS)
+split_count_kernel(SplitArgs a)
+{
+    __shared__ uint32_t s_red[BIN_WARPS];
+    extern __shared__ __align__(16) uint8_t s_done[];   // far: the per-tile "saturated" map, one bit per tile (when it fits)
+    const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t V = a.counters->num_visible;
+    const uint32_t nparts = (V + BIN_PART - 1u) / BIN_PART;
+    const uint32_t cut = a.counters->split_cut;
+    const uint32_t tiles_x = a.uniforms->tiles_x;
+    const uint32_t *bits = nullptr;
+    if (a.far && a.done_in_smem) {
+        pack_done_bits(a.tile_done, tiles_x * a.uniforms->tiles_y, reinterpret_cast<uint32_t *>(s_done));
+        bits = reinterpret_cast<const uint32_t *>(s_done);
+    }
+    for (uint32_t part = blockIdx.x; part < nparts; part += gridDim.x) {
+        const uint32_t first = part * BIN_PART + tid * BIN_SPT;
+        uint32_t k[BIN_SPT];
+        load_keys4(a.keys, first, V, k);
+        uint32_t keep = 0u;                                             // bit j: splat first + j enters the list
+        if (!a.far) {
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) if (first + j < V && k[j] >= cut) keep |= 1u << j;
+        } else {
+            bool cand[BIN_SPT], any = false;
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) { cand[j] = first + j < V && k[j] < cut; any = any || cand[j]; }
+            uint2 rc[BIN_SPT];
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) rc[j] = make_uint2(0u, 0u);
+            if (any) {
+                if (first + BIN_SPT <= V) {
+                    const uint4 *p = reinterpret_cast<const uint4 *>(a.rects + first);   // 32-B aligned: first % 4 == 0
+                    const uint4 q0 = p[0], q1 = p[1];
+                    rc[0] = make_uint2(q0.x, q0.y); rc[1] = make_uint2(q0.z, q0.w); rc[2] = make_uint2(q1.x, q1.y); rc[3] = make_uint2(q1.z, q1.w);
+                } else {
+#pragma unroll
+                    for (int j = 0; j < BIN_SPT; j++) if (cand[j]) rc[j] = a.rects[first + j];
+                }
+            }
+            SplatRects r;
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) {
+                r.slot[j] = first + j;
+                r.xy[j] = rc[j].x;
+                r.w[j] = rc[j].y & 0xffffu;
+                r.h[j] = rc[j].y >> 16;
+                r.cnt[j] = cand[j] ? r.w[j] * r.h[j] : 0u;
+            }
+            const uint32_t keep4 = drop_saturated(tiles_x, r, a.tile_done, bits);
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) keep |= ((keep4 >> (8 * j)) & 1u) << j;
+        }
+        uint32_t b[BIN_SPT], c = 0;
+#pragma unroll
+        for (int j = 0; j < BIN_SPT; j++) { b[j] = __ballot_sync(0xffffffffu, (keep >> j) & 1u); c += (uint32_t)__popc(b[j]); }
+        if (lane == 0) {
+            *reinterpret_cast<uint4 *>(a.keep_bits + (size_t)part * (BIN_WARPS * BIN_SPT) + warp * BIN_SPT) = make_uint4(b[0], b[1], b[2], b[3]);
+            s_red[warp] = c;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            uint32_t t = 0;
+#pragma unroll
+            for (int w = 0; w < BIN_WARPS; w++) t += s_red[w];
+            a.part_counts[part] = t;
+        }
+        __syncthreads();
+    }
+}
+
+// SCAN (one CTA): partition bases and the list length
+__global__ void __launch_bounds__(1024)
+split_scan_kernel(SplitArgs a)
+{
+    const uint32_t V = a.counters->num_visible;
+    const uint32_t nparts = (V + BIN_PART - 1u) / BIN_PART;
+    const uint32_t total = block_exclusive_scan_1024<uint32_t>(a.part_counts, a.part_bases, nparts);   // <= V
+    if (threadIdx.x == 0) *a.count_out = nparts ? total : 0u;
+}
+
+// SCATTER: the kept (key, slot) pairs at their slot-order position in the list + the list's four depth-digit histograms.
+// A splat's rank inside its warp counts the kept splats of the lower lanes (all four of each) and its own earlier ones.
+__global__ void __launch_bounds__(BIN_THREADS)
+split_scatter_kernel(SplitArgs a)
+{
+    __shared__ uint32_t s_hist[4][256];
+    __shared__ uint32_t s_wcnt[BIN_WARPS];
+    const unsigned tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    for (unsigned i = tid; i < 4u * 256u; i += BIN_THREADS) (&s_hist[0][0])[i] = 0u;
+    __syncthreads();
+    const uint32_t V = a.counters->num_visible;
+    const uint32_t nparts = (V + BIN_PART - 1u) / BIN_PART;
+    const uint32_t lt = lanemask_lt();
+    for (uint32_t part = blockIdx.x; part < nparts; part += gridDim.x) {
+        const uint4 wb = *reinterpret_cast<const uint4 *>(a.keep_bits + (size_t)part * (BIN_WARPS * BIN_SPT) + warp * BIN_SPT);
+        const uint32_t b[BIN_SPT] = {wb.x, wb.y, wb.z, wb.w};
+        uint32_t before = 0, total = 0, mine = 0;
+#pragma unroll
+        for (int j = 0; j < BIN_SPT; j++) {
+            before += (uint32_t)__popc(b[j] & lt);
+            total += (uint32_t)__popc(b[j]);
+            mine |= ((b[j] >> lane) & 1u) << j;
+        }
+        if (lane == 0) s_wcnt[warp] = total;
+        __syncthreads();
+        uint32_t pos = __ldg(a.part_bases + part) + before;
+#pragma unroll
+        for (int w = 0; w < BIN_WARPS; w++) if (w < (int)warp) pos += s_wcnt[w];
+        if (mine) {
+            const uint32_t first = part * BIN_PART + tid * BIN_SPT;
+            uint32_t k[BIN_SPT];
+            load_keys4(a.keys, first, V, k);
+#pragma unroll
+            for (int j = 0; j < BIN_SPT; j++) {
+                if ((mine >> j) & 1u) {
+                    a.keys_out[pos] = k[j];
+                    a.vals_out[pos] = first + j;                        // stage 1 compacts in slot order: position == slot
+#pragma unroll
+                    for (int d = 0; d < 4; d++) atomicAdd(&s_hist[d][(k[j] >> (8 * d)) & 255u], 1u);
+                    pos++;
+                }
+            }
+        }
+        __syncthreads();                                                // s_wcnt is rewritten by the next partition
+    }
+    for (unsigned i = tid; i < 4u * 256u; i += BIN_THREADS) {
+        const uint32_t c = (&s_hist[0][0])[i];
+        if (c) atomicAdd(a.hist + i, c);
+    }
+}
+
 }  // namespace
+
+cudaError_t launch_split_cut(const SplitArgs &a, int grid, cudaStream_t stream)
+{
+    split_cut_kernel<<<grid, BIN_THREADS, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_split_compact(const SplitArgs &a, int grid_count, int grid_scatter, cudaStream_t stream)
+{
+    SplitArgs ac = a;
+    const size_t done_bytes = a.far ? done_bits_bytes(a.num_tiles_hint) : 0u;
+    ac.done_in_smem = done_bytes ? 1u : 0u;
+    split_count_kernel<<<grid_count, BIN_THREADS, done_bytes, stream>>>(ac);
+    split_scan_kernel<<<1, 1024, 0, stream>>>(ac);
+    split_scatter_kernel<<<grid_scatter, BIN_THREADS, 0, stream>>>(ac);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_binning(const BinningArgs &a, int grid_count, int grid_expand, cudaStream_t stream)
 {
     // far slab: the tile_done map travels in dynamic shared memory when it fits under the 48 KB default limit
     BinningArgs ac = a;
-    // (one bit per tile + one spare word; up to 16384 x 16384 pixels = 1 Mi tiles = 128 KB would not fit the default 48 KB: above
-    // 256 Ki tiles the kernel reads the byte map from global memory)
-    const size_t done_bytes = (a.tile_done && a.num_tiles_hint && a.num_tiles_hint <= 262144u) ? (((size_t)a.num_tiles_hint + 31u) / 32u + 1u) * 4u : 0u;
+    const size_t done_bytes = a.tile_done ? done_bits_bytes(a.num_tiles_hint) : 0u;
     ac.done_in_smem = done_bytes ? 1u : 0u;
     bin_count_kernel<<<grid_count, BIN_THREADS, done_bytes, stream>>>(ac);
     bin_scan_kernel<<<1, 1024, 0, stream>>>(a);

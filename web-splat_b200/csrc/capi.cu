@@ -674,7 +674,7 @@ extern "C" int32_t ws_pointcloud_dilation_kernel_size(const ws_pointcloud *pc, f
 }
 
 // ------------------------------------------------------------------------------------
-enum { EV_START = 0, EV_PRE, EV_DSORT, EV_BIN, EV_TSORT, EV_BLEND0, EV_BLEND1, EV_NEAR_BLEND, EV_BIN2, EV_TSORT2, EV_COUNT };
+enum { EV_START = 0, EV_PRE, EV_DSORT, EV_BIN, EV_TSORT, EV_BLEND0, EV_BLEND1, EV_NEAR_BLEND, EV_BIN2, EV_TSORT2, EV_DSORT2, EV_COUNT };
 enum { TK_PRE = 0, TK_BIN = 1, TK_DSORT = 2, TK_TSORT = 6, TK_TSORT_FAR = 9 };
 
 struct ShardState {
@@ -717,12 +717,15 @@ struct ws_renderer {
     // device buffers
     FrameUniforms *d_uniforms = nullptr;
     uint8_t *d_scratch = nullptr; size_t scratch_bytes = 0;
+    size_t scratch_bytes_one_sort = 0;     // the scratch without the second set of depth look-back words (frames that sort once)
     FrameCounters *d_counters = nullptr;
-    uint32_t *d_hist_depth = nullptr, *d_hist_tile = nullptr;
+    uint32_t *d_hist_depth = nullptr, *d_hist_tile = nullptr;   // depth: 3 x (4 x 256): stage 1, near list, far survivors
+    uint32_t *d_cut_hist = nullptr;                              // occlusion split: SPLIT_CUT_BINS key-value bins
     uint32_t *d_scan_pre = nullptr, *d_scan_bin = nullptr, *d_part_bases = nullptr, *d_bin_bases = nullptr;
     uint32_t *d_status_depth = nullptr, *d_status_tile = nullptr, *d_gstatus_depth = nullptr, *d_gstatus_tile = nullptr;
     uint32_t *d_splats = nullptr;
     uint32_t *d_keys[2] = {nullptr, nullptr}, *d_vals[2] = {nullptr, nullptr};
+    uint32_t *d_list_keys = nullptr, *d_list_vals = nullptr;    // occlusion split: ping-pong partner of keys[1] / vals[1] for the near / far lists
     uint2 *d_rects = nullptr;
     uint32_t *d_ptiles[2] = {nullptr, nullptr}, *d_pslots[2] = {nullptr, nullptr};
     uint2 *d_ranges = nullptr;
@@ -747,9 +750,11 @@ struct ws_renderer {
     // occlusion split (two depth slabs, nearest first; DESIGN.md section 4)
     int split_mode = 2;                    // 0 off, 1 on, 2 auto (ws_renderer_set_occlusion_split)
     bool frame_split = false;              // the prepared frame was built split
+    bool frame_cut = false;                // ... with the slabs cut by key value (single GPU): no buffer holds the full depth order
     float4 *d_state = nullptr; size_t state_px = 0;   // per pixel {r, g, b, T} after the near slab
     uint8_t *d_tile_done = nullptr;        // per tile: saturated by the near slab
-    uint32_t *d_keep4 = nullptr;           // far slab: one byte per splat, written by bin_count, read by bin_expand
+    uint32_t *d_keep4 = nullptr;           // far slab of a sharded frame: one byte per splat, written by bin_count, read by bin_expand;
+                                           // single GPU: the split's keep bits (one per splat), split_count -> split_scatter
     int tile_out_far = 0;
     cudaStream_t cap_stream = nullptr;
     cudaGraphExec_t prep_exec = nullptr;
@@ -776,6 +781,8 @@ static void free_sort_stuff(ws_renderer *r)
         cudaFree(r->d_ptiles[i]); r->d_ptiles[i] = nullptr;
         cudaFree(r->d_pslots[i]); r->d_pslots[i] = nullptr;
     }
+    cudaFree(r->d_list_keys); r->d_list_keys = nullptr;
+    cudaFree(r->d_list_vals); r->d_list_vals = nullptr;
     cudaFree(r->d_rects); r->d_rects = nullptr;
     cudaFree(r->d_keep4); r->d_keep4 = nullptr;
     r->n_cap = 0; r->pair_cap = 0;
@@ -899,21 +906,27 @@ static ws_status ensure_capacity(ws_renderer *r, uint32_t n, uint32_t tiles)
         const size_t sparts_p = ((size_t)pair_cap + SORT_PART - 1) / SORT_PART;
         size_t off = 0;
         const size_t o_counters = off; off = align_up(off + sizeof(FrameCounters), 256);
-        const size_t o_hd = off; off = align_up(off + 4 * 256 * 4, 256);
+        const size_t o_hd = off; off = align_up(off + 3 * 4 * 256 * 4, 256);  // 4 x 256 for stage 1, the near list, the far survivors
+        const size_t o_hc = off; off = align_up(off + SPLIT_CUT_BINS * 4, 256);
         const size_t o_ht = off; off = align_up(off + 8 * 256 * 4, 256);      // 4 x 256 per slab
         const size_t o_sp = off; off = align_up(off + parts256 * 4, 256);
         const size_t o_sb = off; off = align_up(off + parts256 * 4, 256);
         const size_t o_pb = off; off = align_up(off + parts256 * 4, 256);
         const size_t o_bb = off; off = align_up(off + parts256 * 4, 256);
-        const size_t o_sd = off; off = align_up(off + 4 * sparts_n * 256 * 4, 256);
         const size_t o_st = off; off = align_up(off + 2 * 3 * sparts_p * 256 * 4, 256);     // x2: one set per depth slab
         const size_t gparts_n = (sparts_n + SORT_LB_GROUP - 1) / SORT_LB_GROUP, gparts_p = (sparts_p + SORT_LB_GROUP - 1) / SORT_LB_GROUP;
-        const size_t o_gd = off; off = align_up(off + 4 * gparts_n * 256 * 4, 256);
+        const size_t o_gd = off; off = align_up(off + 2 * 4 * gparts_n * 256 * 4, 256);
         const size_t o_gt = off; off = align_up(off + 2 * 3 * gparts_p * 256 * 4, 256);
+        // x2: near list, far survivors (split frame on one GPU); the second set is last, so that the other frames leave it
+        // out of the per-frame clear
+        const size_t o_sd = off; off = off + 4 * sparts_n * 256 * 4;
+        r->scratch_bytes_one_sort = off;
+        off = align_up(off + 4 * sparts_n * 256 * 4, 256);
         CU(cudaMalloc(&r->d_scratch, off));
         r->scratch_bytes = off;
         r->d_counters = reinterpret_cast<FrameCounters *>(r->d_scratch + o_counters);
         r->d_hist_depth = reinterpret_cast<uint32_t *>(r->d_scratch + o_hd);
+        r->d_cut_hist = reinterpret_cast<uint32_t *>(r->d_scratch + o_hc);
         r->d_hist_tile = reinterpret_cast<uint32_t *>(r->d_scratch + o_ht);
         r->d_scan_pre = reinterpret_cast<uint32_t *>(r->d_scratch + o_sp);
         r->d_scan_bin = reinterpret_cast<uint32_t *>(r->d_scratch + o_sb);
@@ -930,8 +943,12 @@ static ws_status ensure_capacity(ws_renderer *r, uint32_t n, uint32_t tiles)
             CU(cudaMalloc(&r->d_ptiles[i], (size_t)pair_cap * 4));
             CU(cudaMalloc(&r->d_pslots[i], (size_t)pair_cap * 4));
         }
+        CU(cudaMalloc(&r->d_list_keys, nn * 4));
+        CU(cudaMalloc(&r->d_list_vals, nn * 4));
         CU(cudaMalloc(&r->d_rects, nn * 8));
-        CU(cudaMalloc(&r->d_keep4, (nn + 2 * 1024 + 4) / 4 * 4 + 4096));   // one byte per far-slab splat (the far slab may be most of the cloud), rounded up to whole 1024-splat partitions
+        // one byte per far-slab splat (the far slab may be most of the cloud), rounded up to whole 1024-splat partitions;
+        // also holds the split's keep bits (one bit per splat, 128 B per partition)
+        CU(cudaMalloc(&r->d_keep4, (nn + 2 * 1024 + 4) / 4 * 4 + 4096));
         r->n_cap = n; r->pair_cap = pair_cap;
         r->buf_generation = next_generation();
     }
@@ -1000,6 +1017,7 @@ static ws_status validate_frame(ws_renderer *r, ws_pointcloud *pc, const ws_spla
 static ws_status decide_split(ws_renderer *r, uint64_t points_here, uint32_t W, uint32_t H)
 {
     r->frame_split = r->split_mode == 1 || (r->split_mode == 2 && points_here >= 2000000u);
+    r->frame_cut = r->frame_split && r->shard.world == 0;   // one GPU: the slabs are cut by key value (enqueue_stage2)
     if (r->frame_split) {
         const size_t px = (size_t)W * H;
         if (r->state_px < px) {
@@ -1042,49 +1060,57 @@ static ws_status begin_frame(ws_renderer *r, ws_pointcloud *pc, const ws_splatti
     // pageable source: the runtime stages the 0.5 KB before returning, so h_uniforms may be reused
     CU(cudaMemcpyAsync(r->d_uniforms, &U, sizeof U, cudaMemcpyHostToDevice, stream));
     if (with_clears) {
-        CU(cudaMemsetAsync(r->d_scratch, 0, r->scratch_bytes, stream));
+        CU(cudaMemsetAsync(r->d_scratch, 0, r->frame_cut ? r->scratch_bytes : r->scratch_bytes_one_sort, stream));
         CU(cudaMemsetAsync(r->d_ranges, 0xff, (size_t)r->tiles_cap * 8 * (r->frame_split ? 2 : 1), stream));    // {begin, ~end} identities for atomicMin (one set per depth slab)
     }
     return WS_OK;
 }
 
-// stage 2: depth passes on the V visible splats, tile binning, tile-id passes (+ ranges)
+// stage 2: depth passes on the V visible splats, tile binning, tile-id passes (+ ranges).  A split frame on one GPU
+// depth-sorts only the near list and the far survivors instead of all V splats (binning.cu: split_*).
 static ws_status enqueue_stage2(ws_renderer *r, cudaStream_t stream)
 {
-    {   // ---- stage 2a
-        const size_t sparts_n = ((size_t)(r->n_cap ? r->n_cap : 1) + SORT_PART - 1) / SORT_PART;
+    // ---- stage 2a: the four depth-digit passes over a (key, slot) list of *n_ptr pairs, ping-ponging between keys[0] /
+    //      vals[0] and keys[1] / vals[1]; `set` selects one of two sets of look-back status words and tickets (the far
+    //      survivors of a split frame are sorted with the second set, the frame's first sort with the first)
+    const size_t sparts_n = ((size_t)(r->n_cap ? r->n_cap : 1) + SORT_PART - 1) / SORT_PART;
+    const size_t gparts_n = (sparts_n + SORT_LB_GROUP - 1) / SORT_LB_GROUP;
+    auto depth_sort = [&](uint32_t *const keys[2], uint32_t *const vals[2], const uint32_t *n_ptr, const uint32_t *hist,
+                          uint32_t *tickets, int set, int *out) -> ws_status {
         int src = 0;
         for (int p = 0; p < r->depth_passes; p++) {
             SortPassArgs a;
-            a.keys_in = r->d_keys[src]; a.vals_in = r->d_vals[src];
-            a.keys_out = r->d_keys[src ^ 1]; a.vals_out = r->d_vals[src ^ 1];
-            a.n_ptr = &r->d_counters->num_visible; a.n_cap = r->n_cap;
-            a.status = r->d_status_depth + (size_t)p * sparts_n * 256;
-            a.gstatus = r->d_gstatus_depth + (size_t)p * ((sparts_n + SORT_LB_GROUP - 1) / SORT_LB_GROUP) * 256;
+            a.keys_in = keys[src]; a.vals_in = vals[src];
+            a.keys_out = keys[src ^ 1]; a.vals_out = vals[src ^ 1];
+            a.n_ptr = n_ptr; a.n_cap = r->n_cap;
+            a.status = r->d_status_depth + ((size_t)set * 4 + p) * sparts_n * 256;
+            a.gstatus = r->d_gstatus_depth + ((size_t)set * 4 + p) * gparts_n * 256;
             a.ranges = nullptr;
-            a.ticket = &r->d_counters->ticket[TK_DSORT + p];
-            a.hist = r->d_hist_depth + p * 256;
+            a.ticket = tickets + p;
+            a.hist = hist + p * 256;
             a.shift = 8u * (uint32_t)p;
             a.err = &r->d_counters->error_flags;
             CU(launch_sort_pass(a, r->grid_sort, stream));
             src ^= 1;
         }
-        r->depth_out = src;
-    }
-    if (r->timing) CU(cudaEventRecord(r->ev[EV_DSORT], stream));
-    // ---- stage 2b + 2c for one slab of the depth-sorted splats: expand into (tile, slot) pairs in depth order, then the
-    //      tile-id passes on those pairs.  `half` selects the slab's private set of look-back status words, digit
-    //      histograms, tickets and tile ranges (the pair buffers themselves are reused: the slabs run back to back).
-    auto bin_and_tile_sort = [&](uint32_t slab, int half, int ev_bin, int ev_tsort, int *tile_out) -> ws_status {
+        *out = src;
+        return WS_OK;
+    };
+    // ---- stage 2b + 2c for one slab of the depth-sorted splats (`sorted_slots`: [0, *list_len), or the position range
+    //      slab_bounds gives when list_len is NULL): expand into (tile, slot) pairs in depth order, then the tile-id
+    //      passes on those pairs.  `half` selects the slab's private set of look-back status words, digit histograms,
+    //      tickets and tile ranges (the pair buffers themselves are reused: the slabs run back to back).
+    auto bin_and_tile_sort = [&](uint32_t slab, int half, int ev_bin, int ev_tsort, int *tile_out,
+                                 const uint32_t *sorted_slots, const uint32_t *list_len) -> ws_status {
         const size_t sparts_p = ((size_t)r->pair_cap + SORT_PART - 1) / SORT_PART;
         const size_t gparts_p = (sparts_p + SORT_LB_GROUP - 1) / SORT_LB_GROUP;
         // each slab has its own set of look-back status words (the second set starts after the 3 passes of the first)
         const size_t set_off = half ? 3 * sparts_p : 0, gset_off = half ? 3 * gparts_p : 0;
         const uint32_t cap = r->pair_cap;
-        uint32_t *num_pairs = (slab == 1u) ? &r->d_counters->num_pairs_near : &r->d_counters->num_pairs;
+        uint32_t *num_pairs = (r->frame_split && !half) ? &r->d_counters->num_pairs_near : &r->d_counters->num_pairs;
         {
             BinningArgs a;
-            a.sorted_slots = r->d_vals[r->depth_out]; a.rects = r->d_rects; a.uniforms = r->d_uniforms;
+            a.sorted_slots = sorted_slots; a.list_len = list_len ? list_len : &r->d_counters->num_visible; a.rects = r->d_rects; a.uniforms = r->d_uniforms;
             a.counters = r->d_counters; a.pair_tiles = r->d_ptiles[0]; a.pair_slots = r->d_pslots[0];
             a.part_counts = r->d_scan_bin; a.part_bases = r->d_bin_bases; a.hist = r->d_hist_tile + half * 4 * 256;
             a.slab = slab; a.tile_done = (slab == 2u) ? r->d_tile_done : nullptr; a.pair_cap = cap; a.num_pairs_out = num_pairs;
@@ -1116,12 +1142,40 @@ static ws_status enqueue_stage2(ws_renderer *r, cudaStream_t stream)
         if (r->timing) CU(cudaEventRecord(r->ev[ev_tsort], stream));
         return WS_OK;
     };
-    if (!r->frame_split) return bin_and_tile_sort(0u, 0, EV_BIN, EV_TSORT, &r->tile_out);
-
-    // ---- occlusion split: near slab -> composite into per-pixel state + per-tile saturation -> far slab, whose
-    //      binning drops every splat that only touches saturated tiles (most of them: a tile needs ~1/5 of its list)
-    ws_status st = bin_and_tile_sort(1u, 0, EV_BIN, EV_TSORT, &r->tile_out);
+    ws_status st;
+    // r->frame_cut (decide_split): a split frame on one GPU never sorts all V splats, the slabs are cut by key value.  Sharded
+    // frames keep the full sort and the cut by position (their receive buffers are laid out by the exchange, not in slot order).
+    SplitArgs sa;
+    memset(&sa, 0, sizeof sa);
+    uint32_t *const lkeys[2] = {r->d_keys[1], r->d_list_keys}, *const lvals[2] = {r->d_vals[1], r->d_list_vals};
+    if (!r->frame_cut) {
+        st = depth_sort(r->d_keys, r->d_vals, &r->d_counters->num_visible, r->d_hist_depth, &r->d_counters->ticket[TK_DSORT], 0, &r->depth_out);
+        if (st != WS_OK) return st;
+        if (r->timing) CU(cudaEventRecord(r->ev[EV_DSORT], stream));
+        if (!r->frame_split) return bin_and_tile_sort(0u, 0, EV_BIN, EV_TSORT, &r->tile_out, r->d_vals[r->depth_out], nullptr);
+        st = bin_and_tile_sort(1u, 0, EV_BIN, EV_TSORT, &r->tile_out, r->d_vals[r->depth_out], nullptr);
+    } else {
+        // cut (a key value near the near_pct quantile) -> near list (key >= cut, slot order) into keys[1] / vals[1] ->
+        // its depth sort (4 passes: the result is back in keys[1] / vals[1]); keys[0] / vals[0] stay in slot order
+        sa.keys = r->d_keys[0]; sa.rects = r->d_rects; sa.uniforms = r->d_uniforms; sa.counters = r->d_counters;
+        sa.cut_hist = r->d_cut_hist; sa.near_pct = split_near_pct();
+        sa.num_tiles_hint = r->h_uniforms.tiles_x * r->h_uniforms.tiles_y;
+        sa.part_counts = r->d_scan_bin; sa.part_bases = r->d_bin_bases; sa.keep_bits = r->d_keep4;
+        sa.keys_out = lkeys[0]; sa.vals_out = lvals[0];
+        CU(launch_split_cut(sa, r->ctx->sm_count * 2, stream));
+        sa.far = 0; sa.hist = r->d_hist_depth + 4 * 256; sa.count_out = &r->d_counters->num_near;
+        CU(launch_split_compact(sa, r->ctx->sm_count * 8, r->ctx->sm_count * 4, stream));
+        int out = 0;
+        st = depth_sort(lkeys, lvals, &r->d_counters->num_near, sa.hist, &r->d_counters->ticket[TK_DSORT], 0, &out);
+        if (st != WS_OK) return st;
+        if (out != 0) return fail(WS_ERR_UNSUPPORTED, "internal: odd number of depth passes");
+        if (r->timing) CU(cudaEventRecord(r->ev[EV_DSORT], stream));
+        st = bin_and_tile_sort(0u, 0, EV_BIN, EV_TSORT, &r->tile_out, lvals[0], &r->d_counters->num_near);
+    }
     if (st != WS_OK) return st;
+
+    // ---- occlusion split: near slab -> composite into per-pixel state + per-tile saturation -> far slab, of which only
+    //      the splats that touch an unsaturated tile are binned (a tile needs ~1/5 of its list)
     {
         CompositeArgs a;
         memset(&a, 0, sizeof a);
@@ -1135,18 +1189,29 @@ static ws_status enqueue_stage2(ws_renderer *r, cudaStream_t stream)
         if (rows) CU(launch_composite(a, r->h_uniforms.tiles_x, rows, stream));
     }
     if (r->timing) CU(cudaEventRecord(r->ev[EV_NEAR_BLEND], stream));
-    return bin_and_tile_sort(2u, 1, EV_BIN2, EV_TSORT2, &r->tile_out_far);
+    if (!r->frame_cut)      // far slab by position: bin_count drops the splats whose tiles are all saturated
+        return bin_and_tile_sort(2u, 1, EV_BIN2, EV_TSORT2, &r->tile_out_far, r->d_vals[r->depth_out], nullptr);
+    // far cull in slot order (coalesced keys + rectangles) -> survivors into keys[1] / vals[1] (the near list is binned
+    // by now) -> their depth sort -> binned with no further filter
+    sa.far = 1; sa.tile_done = r->d_tile_done; sa.hist = r->d_hist_depth + 2 * 4 * 256; sa.count_out = &r->d_counters->num_far;
+    CU(launch_split_compact(sa, r->ctx->sm_count * 8, r->ctx->sm_count * 4, stream));
+    int out = 0;
+    st = depth_sort(lkeys, lvals, &r->d_counters->num_far, sa.hist, r->d_counters->ticket_far, 1, &out);
+    if (st != WS_OK) return st;
+    if (r->timing) CU(cudaEventRecord(r->ev[EV_DSORT2], stream));
+    return bin_and_tile_sort(0u, 1, EV_BIN2, EV_TSORT2, &r->tile_out_far, lvals[0], &r->d_counters->num_far);
 }
 
 // clears + stage 1 + stage 2 of the plain (single-GPU) frame, on `stream`
 static ws_status enqueue_prepare_body(ws_renderer *r, ws_pointcloud *pc, cudaStream_t stream)
 {
     const FrameUniforms &U = r->h_uniforms;
-    CU(cudaMemsetAsync(r->d_scratch, 0, r->scratch_bytes, stream));
+    CU(cudaMemsetAsync(r->d_scratch, 0, r->frame_cut ? r->scratch_bytes : r->scratch_bytes_one_sort, stream));
     CU(cudaMemsetAsync(r->d_ranges, 0xff, (size_t)r->tiles_cap * 8 * (r->frame_split ? 2 : 1), stream));    // {begin, ~end} identities for atomicMin
     if (r->timing) CU(cudaEventRecord(r->ev[EV_START], stream));
     {   // ---- stage 1
         PreprocessArgs a;
+        a.key_range = r->frame_cut ? 1u : 0u;                  // the cut needs the min / max of the keys
         a.gaussians = pc->d_gaussians; a.xyz = pc->d_xyz; a.sh_coefs = pc->d_sh; a.covars = pc->d_covars;
         a.uniforms = r->d_uniforms;
         a.splats = r->d_splats; a.depth_keys = r->d_keys[0]; a.slot_vals = r->d_vals[0]; a.rects = r->d_rects;
@@ -1358,12 +1423,13 @@ extern "C" ws_status ws_renderer_shard_begin(ws_renderer *r, ws_pointcloud *pc, 
     if (pc->n > s.local_cap) return fail(WS_ERR_INVALID_ARGUMENT, "local shard larger than configured");
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     CU(cudaSetDevice(r->ctx->device));
-    r->frame_split = false;
+    r->frame_split = false; r->frame_cut = false;
     st = begin_frame(r, pc, args, s.recv_cap, stream);
     if (st != WS_OK) return st;
     if (r->timing) CU(cudaEventRecord(r->ev[EV_START], stream));
     {   // ---- stage 1 on the local shard, into the local staging arrays
         PreprocessArgs a;
+        a.key_range = 0u;
         a.gaussians = pc->d_gaussians; a.xyz = pc->d_xyz; a.sh_coefs = pc->d_sh; a.covars = pc->d_covars;
         a.uniforms = r->d_uniforms;
         a.splats = s.l_splats; a.depth_keys = s.l_keys; a.slot_vals = s.l_vals; a.rects = s.l_rects;
@@ -1454,13 +1520,14 @@ extern "C" ws_status ws_renderer_shard_frame_to_root(ws_renderer *r, ws_pointclo
     // everything of the frame that does not depend on the frame's content: clears, epoch, stage 1, routing + exchange,
     // stage 2, the band compositor (pixels into the root's frame of this parity), the root's wait for all bands
     auto body = [&](cudaStream_t q) -> ws_status {
-        CU(cudaMemsetAsync(r->d_scratch, 0, r->scratch_bytes, q));
+        CU(cudaMemsetAsync(r->d_scratch, 0, r->frame_cut ? r->scratch_bytes : r->scratch_bytes_one_sort, q));
         CU(cudaMemsetAsync(r->d_ranges, 0xff, (size_t)r->tiles_cap * 8 * (r->frame_split ? 2 : 1), q));
         CU(cudaMemsetAsync(s.hist_dummy, 0, 4 * 256 * 4, q));
         CU(launch_epoch_advance(s.d_epoch, q));
         if (r->timing) CU(cudaEventRecord(r->ev[EV_START], q));
         {   // stage 1 on the local shard
             PreprocessArgs a;
+            a.key_range = 0u;
             a.gaussians = pc->d_gaussians; a.xyz = pc->d_xyz; a.sh_coefs = pc->d_sh; a.covars = pc->d_covars;
             a.uniforms = r->d_uniforms;
             a.splats = s.l_splats; a.depth_keys = s.l_keys; a.slot_vals = s.l_vals; a.rects = s.l_rects;
@@ -1699,8 +1766,13 @@ extern "C" ws_status ws_renderer_stats(ws_renderer *r, ws_frame_stats *s)
         s->ms_tile_sort = el(EV_BIN, EV_TSORT);
         s->ms_ranges = 0.f;                                   // fused into the last tile-sort pass
         if (r->rendered) s->ms_blend = el(EV_BLEND0, EV_BLEND1);
-        if (r->frame_split) {                                 // near slab | near composite | far slab ... far composite
-            s->ms_binning += el(EV_NEAR_BLEND, EV_BIN2);
+        if (r->frame_split) {                                 // near slab | near composite | [far cull + survivor sort] far slab ... far composite
+            if (r->frame_cut) {
+                s->ms_depth_sort += el(EV_NEAR_BLEND, EV_DSORT2);
+                s->ms_binning += el(EV_DSORT2, EV_BIN2);
+            } else {
+                s->ms_binning += el(EV_NEAR_BLEND, EV_BIN2);
+            }
             s->ms_tile_sort += el(EV_BIN2, EV_TSORT2);
             s->ms_blend += el(EV_TSORT, EV_NEAR_BLEND);
         }
@@ -1716,10 +1788,16 @@ extern "C" ws_status ws_renderer_stats(ws_renderer *r, ws_frame_stats *s)
     s->bytes_preprocess = N * 12 + N * rec + V * shb + V * (20 + 4 + 4 + 8);   // count (xyz plane) + main
     s->bytes_sort = (uint64_t)r->depth_passes * V * 16 + V * 12 + P * 8 + (uint64_t)r->tile_passes * P * 16 + T * 8;
     s->bytes_blend = P * 24 + T * 8 + (uint64_t)U.width * U.height * bytes_per_pixel(r->format);
-    if (r->frame_split) {                                         // the far slab re-reads the slots + rectangles, the state goes out and in
+    if (r->frame_cut) {
+        // the keys actually sorted and binned are the near list + the far survivors; the cut histogram and the near
+        // compaction read the V keys twice (keys + slots written for the list), the far cull reads keys + rectangles
+        const uint64_t L = (uint64_t)c.num_near + c.num_far;
+        s->bytes_sort = (uint64_t)r->depth_passes * L * 16 + L * 12 + P * 8 + (uint64_t)r->tile_passes * P * 16 + T * 8;
+        s->bytes_sort += V * 4 + V * 4 + V * 12 + L * 12;
+    } else if (r->frame_split) {                                  // the far slab re-reads the slots + rectangles
         s->bytes_sort += (V - V / 4) * 12;
-        s->bytes_blend += T * 8 + (uint64_t)U.width * U.height * 32;
     }
+    if (r->frame_split) s->bytes_blend += T * 8 + (uint64_t)U.width * U.height * 32;   // the state goes out and in
     if (c.error_flags) return fail(WS_ERR_CUDA, (c.error_flags & 2u) ? "sharded frame: receive capacity exceeded" : ((c.error_flags & 4u) ? "sharded frame: a peer never arrived" : "internal: decoupled look-back watchdog fired"));
     if (c.pair_overflow) return fail(WS_ERR_PAIR_OVERFLOW, "pair capacity exceeded; raise it with ws_renderer_set_pair_capacity");
     return WS_OK;
@@ -1753,6 +1831,27 @@ extern "C" ws_status ws_renderer_read_buffer(ws_renderer *r, ws_buffer_id which,
     }
     if (written) *written = bytes;
     if (dst_bytes < bytes) return fail(WS_ERR_INVALID_ARGUMENT, "destination too small");
+    if (r->frame_cut && (which == WS_BUF_DEPTH_KEYS || which == WS_BUF_SORTED_KEYS || which == WS_BUF_SORTED_INDICES)) {
+        // a split frame sorted only its near list and far survivors; keys[0] / vals[0] still hold the slot-order keys and
+        // slots of stage 1, so the complete stable order of all V splats is computed here, synchronously (debug path)
+        if (which == WS_BUF_DEPTH_KEYS) {
+            if (V) CU(cudaMemcpy(dst, r->d_keys[0], V * 4, cudaMemcpyDeviceToHost));
+            return WS_OK;
+        }
+        if (!V) return WS_OK;
+        uint32_t *dk = nullptr, *dv = nullptr;
+        CU(cudaMalloc(&dk, V * 4));
+        cudaError_t e = cudaMalloc(&dv, V * 4);
+        if (e == cudaSuccess) e = cudaMemcpy(dk, r->d_keys[0], V * 4, cudaMemcpyDeviceToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy(dv, r->d_vals[0], V * 4, cudaMemcpyDeviceToDevice);
+        ws_status s = (e == cudaSuccess) ? ws_sort_pairs_u32(r->ctx, dk, dv, (uint32_t)V, 32, nullptr) : fail_cuda(e, "read_buffer: depth order");
+        if (s == WS_OK) {
+            e = cudaMemcpy(dst, which == WS_BUF_SORTED_KEYS ? dk : dv, V * 4, cudaMemcpyDeviceToHost);
+            if (e != cudaSuccess) s = fail_cuda(e, "read_buffer: depth order");
+        }
+        cudaFree(dk); cudaFree(dv);
+        return s;
+    }
     if (which == WS_BUF_DEPTH_KEYS) {
         // un-permute on the host: key_of_slot[sorted_idx[i]] = sorted_key[i]
         std::vector<uint32_t> sk(V), si(V);

@@ -342,6 +342,7 @@ count_kernel(PreprocessArgs a)
 {
     __shared__ FrameUniforms s_u;
     __shared__ uint32_t s_hist[4 * 256];
+    __shared__ uint32_t s_kmax, s_kmin_inv;
     const unsigned tid = threadIdx.x;
     {
         const uint32_t *src = reinterpret_cast<const uint32_t *>(a.uniforms);
@@ -349,7 +350,9 @@ count_kernel(PreprocessArgs a)
         for (unsigned i = tid; i < sizeof(FrameUniforms) / 4u; i += PP_THREADS) dst[i] = src[i];
     }
     for (unsigned i = tid; i < 4u * 256u; i += PP_THREADS) s_hist[i] = 0u;
+    if (tid == 0) { s_kmax = 0u; s_kmin_inv = 0u; }
     __syncthreads();
+    uint32_t kmax = 0u, kmin_inv = 0u;                                     // key range of the survivors (occlusion split's cut)
     const FrameUniforms &U = s_u;
     const uint32_t n = U.num_points;
     const uint32_t nparts = (n + PP_THREADS - 1u) / PP_THREADS;
@@ -388,13 +391,22 @@ count_kernel(PreprocessArgs a)
             if (keep[u]) {
 #pragma unroll
                 for (int d = 0; d < NDIG; d++) atomicAdd(&s_hist[d * 256 + ((key[u] >> (8 * d)) & 255u)], 1u);
+                if (a.key_range) { kmax = max(kmax, key[u]); kmin_inv = max(kmin_inv, ~key[u]); }
             }
         }
+    }
+    if (a.key_range) {
+        kmax = __reduce_max_sync(0xffffffffu, kmax); kmin_inv = __reduce_max_sync(0xffffffffu, kmin_inv);
+        if ((tid & 31u) == 0u) { atomicMax(&s_kmax, kmax); atomicMax(&s_kmin_inv, kmin_inv); }
     }
     __syncthreads();
     for (unsigned i = tid; i < (unsigned)NDIG * 256u; i += PP_THREADS) {
         const uint32_t c = s_hist[i];
         if (c) atomicAdd(a.hist + i, c);
+    }
+    if (tid == 0 && a.key_range) {
+        if (s_kmax) atomicMax(&a.counters->key_max, s_kmax);
+        if (s_kmin_inv) atomicMax(&a.counters->key_min_inv, s_kmin_inv);
     }
 }
 

@@ -55,6 +55,14 @@ struct FrameCounters {
     uint32_t scatter_done;      // sharded mode: CTAs of the exchange kernel that have finished (last one signals the peers)
     uint32_t composite_done;    // sharded mode: CTAs of the band compositor that have finished
     uint32_t num_pairs_near;    // occlusion split: pairs of the near slab (num_pairs then counts the far slab's)
+    // occlusion split on one GPU (binning.cu: split_*): the slabs are cut by depth-key VALUE, not by sorted position
+    uint32_t key_max;           // largest depth key of the visible splats (stage 1 count kernel)
+    uint32_t key_min_inv;       // ~smallest depth key (atomicMax of ~key: the per-frame memset is the identity)
+    uint32_t split_cut;         // near list = visible splats with key >= split_cut
+    uint32_t num_near;          // length of the near list
+    uint32_t num_far;           // far splats that survive the cull against the saturated tiles
+    uint32_t cut_done;          // CTAs of the cut histogram that have finished (the last one picks the cut)
+    uint32_t ticket_far[4];     // depth passes over the far survivors
 };
 
 constexpr int TILE = 16;                    // 16x16 pixel tiles

@@ -24,6 +24,7 @@ struct PreprocessArgs {
     uint32_t *part_bases;         // ceil(N/256): exclusive scan of part_counts (scan kernel)
     uint32_t *hist;               // 4 x 256 depth-key digit histograms (zeroed per frame)
     FrameCounters *counters;
+    uint32_t key_range;           // 1: the count kernel also reduces the min / max of the visible keys (occlusion split's cut)
 };
 cudaError_t launch_preprocess(const PreprocessArgs &a, bool compressed, int grid_count, int grid_main, cudaStream_t stream);
 int preprocess_blocks_per_sm(bool compressed);
@@ -74,9 +75,35 @@ struct BinningArgs {
     uint32_t near_pct;            // occlusion split: share of the depth-sorted splats in the near slab, in percent (0 = the default quarter)
     uint32_t num_tiles_hint;      // host-known number of tiles (sizes the shared-memory copy of tile_done); 0 = unknown
     uint32_t done_in_smem;        // set by launch_binning
+    const uint32_t *list_len;     // device: length of sorted_slots (&counters->num_visible, or the near list / far survivors: slab 0)
 };
 cudaError_t launch_binning(const BinningArgs &a, int grid_count, int grid_expand, cudaStream_t stream);
 int binning_blocks_per_sm();
+
+// ---- occlusion split on one GPU: cut the visible splats by depth-key value, compact the near list, cull the far ones ----
+struct SplitArgs {
+    const uint32_t *keys;         // V depth keys in slot order (stage 1; read only)
+    const uint2 *rects;           // per slot
+    const FrameUniforms *uniforms;
+    FrameCounters *counters;      // reads num_visible, key_max / key_min_inv, split_cut; writes split_cut, cut_done
+    uint32_t *cut_hist;           // SPLIT_CUT_BINS counts of (key - kmin) >> s (zeroed per frame)
+    uint32_t near_pct;            // share of the visible splats the near list should hold, in percent (0 = a quarter)
+    uint32_t far;                 // 0: near list (key >= cut); 1: far survivors (key < cut, tiles not all saturated)
+    const uint8_t *tile_done;     // far: per-tile "saturated by the near slab" bytes (allocation padded to 32 B)
+    uint32_t num_tiles_hint;      // host-known number of tiles (sizes the bit map in shared memory)
+    uint32_t done_in_smem;        // set by launch_split_compact
+    uint32_t *part_counts;        // ceil(V/1024): list entries per partition
+    uint32_t *part_bases;         // ceil(V/1024): exclusive scan
+    uint32_t *keep_bits;          // 32 words per 1024-splat partition: count kernel -> scatter kernel
+    uint32_t *keys_out, *vals_out;   // the compacted (key, slot) list, slot order
+    uint32_t *hist;               // 4 x 256 depth-digit histograms of the list (zeroed per frame)
+    uint32_t *count_out;          // device: length of the list
+};
+constexpr int SPLIT_CUT_BINS = 2048;
+// histogram of the V keys + the cut (last CTA); no host synchronisation, every size read from device memory
+cudaError_t launch_split_cut(const SplitArgs &a, int grid, cudaStream_t stream);
+// count -> scan -> scatter of the near list (a.far == 0) or of the far survivors (a.far == 1)
+cudaError_t launch_split_compact(const SplitArgs &a, int grid_count, int grid_scatter, cudaStream_t stream);
 
 // ---- stage 3 -----------------------------------------------------------------------
 struct CompositeArgs {
