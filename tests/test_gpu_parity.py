@@ -12,70 +12,10 @@ import os
 import numpy as np
 import pytest
 
-from helpers import image_close, make_args, make_generic, oracle_pairs
+from helpers import check_all_stages, frame, image_close, make_args, make_generic
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-
-
-def _frame(ws, ctx, cloud, pos, rot, W, H, fmt=None, clear=(0, 0, 0, 0), split=False, **kw):
-    """One frame through the C ABI.  split=False: one binning + tile sort over all pairs, so that the pair-list
-    read-backs and num_pairs are the complete ones the oracle produces (the occlusion split, on by default in the
-    product, emits fewer pairs for the same image: test_occlusion_split_is_bit_identical)."""
-    import torch
-    fmt = ws.FORMAT_RGBA32_FLOAT if fmt is None else fmt
-    fovx, fovy = ws.synth.fov_for_viewport(W, H)
-    pc = ws.PointCloud.new(ctx, make_generic(ws, cloud))
-    r = ws.GaussianRenderer.new(ctx, fmt, cloud["sh_deg"], cloud["compressed"])
-    r.set_occlusion_split(split)
-    args = make_args(ws, cloud, pos, rot, W, H, fovx, fovy, **kw)
-    r.prepare(None, pc, args)
-    dt = {0: torch.uint8, 1: torch.float16, 2: torch.float32}[fmt]
-    target = torch.empty((H, W, 4), dtype=dt, device="cuda")
-    r.render(target, pc, clear)
-    torch.cuda.synchronize()
-    return r, pc, target.cpu().numpy(), (fovx, fovy)
-
-
-def _check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H, **kw):
-    r, pc, img, (fovx, fovy) = _frame(ws, ctx, cloud, pos, rot, W, H, **kw)
-    ref = orc.render_frame(cloud, pos, rot, W, H, fovx, fovy, want_sens=True, **kw)
-    st = r.stats()
-    V = len(ref["keys"])
-    # uniforms as the reference would upload them
-    assert np.array_equal(r.camera_uniform().view(np.uint32), np.frombuffer(bytes(ref["cam"]), np.uint32))
-    assert r.settings_uniform().tobytes() == bytes(ref["settings"])
-    # stage 1
-    assert st["num_visible"] == V == r.num_visible_points()
-    splats = r.read_buffer(ws.BUF_SPLATS_2D)
-    a, b = splats, ref["splats"]
-    nan_a = np.isnan(a.view(np.float16)); nan_b = np.isnan(b.view(np.float16))
-    assert np.array_equal(nan_a, nan_b)
-    assert np.array_equal(a[~nan_a], b[~nan_b]), "stage-1 halves differ from the oracle"
-    assert np.array_equal(r.read_buffer(ws.BUF_DEPTH_KEYS), ref["keys"])
-    # stage 2 (depth sort)
-    sk, order = orc.sort_pairs(ref["keys"], np.arange(V, dtype=np.uint32))
-    assert np.array_equal(r.read_buffer(ws.BUF_SORTED_KEYS), sk)
-    assert np.array_equal(r.read_buffer(ws.BUF_SORTED_INDICES), order)
-    # tile binning
-    tiles, slots, rects, P = oracle_pairs(orc, ref["splats"], order, W, H)
-    assert st["num_pairs"] == P
-    rc = r.read_buffer(ws.BUF_TILE_RECTS).astype(np.int32)
-    mine = np.stack([rc[:, 0], rc[:, 1], rc[:, 0] + rc[:, 2] - 1, rc[:, 1] + rc[:, 3] - 1], 1)
-    empty = rc[:, 2] == 0
-    assert np.array_equal(empty, rects[:, 2] < rects[:, 0])
-    assert np.array_equal(mine[~empty], rects[~empty])
-    assert np.array_equal(r.read_buffer(ws.BUF_PAIR_TILES), tiles)
-    assert np.array_equal(r.read_buffer(ws.BUF_PAIR_SLOTS), slots)
-    rng_ = r.read_buffer(ws.BUF_TILE_RANGES)
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    cnt = np.bincount(tiles, minlength=T)
-    assert np.array_equal(rng_[:, 1] - rng_[:, 0], cnt)
-    # stage 3
-    d, ok = image_close(img, ref["image"], ref["sens"])
-    assert ok.all(), "image: %d px outside tolerance, max |d| %.3g" % ((~ok).sum(), d.max())
-    assert np.abs(img - ref["image"]).mean() <= 2e-5
-    return r, st, d
 
 
 def test_sort_kat_from_reference(ws, ctx):
@@ -113,7 +53,7 @@ def test_golden_frame(ws, orc, ctx):
     cloud = ws.synth.make_cloud(int(z["n"]), int(z["seed"]))
     pos, rot = ws.synth.orbit_camera(float(z["az"]))
     W, H = int(z["W"]), int(z["H"])
-    r, pc, img, _ = _frame(ws, ctx, cloud, pos, rot, W, H)
+    r, pc, img, _ = frame(ws, ctx, cloud, pos, rot, W, H)
     assert np.array_equal(r.read_buffer(ws.BUF_SPLATS_2D), z["splats"])
     assert np.array_equal(r.read_buffer(ws.BUF_DEPTH_KEYS), z["keys"])
     assert np.array_equal(r.read_buffer(ws.BUF_SORTED_INDICES), z["order"])
@@ -125,7 +65,7 @@ def test_golden_frame(ws, orc, ctx):
 def test_all_stages_small(ws, orc, ctx, n, W, H, az):
     cloud = ws.synth.make_cloud(n, 100 + n)
     pos, rot = ws.synth.orbit_camera(az)
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H)
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H)
 
 
 def test_cfg1_full(ws, orc, ctx):
@@ -133,23 +73,23 @@ def test_cfg1_full(ws, orc, ctx):
     n, W, H, seed, _ = ws.synth.CONFIGS["cfg1"]
     cloud = ws.synth.make_cloud(n, seed)
     pos, rot = ws.synth.fixed_camera()
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H)
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H)
 
 
 @pytest.mark.parametrize("deg", [0, 1, 2])
 def test_lower_sh_degree(ws, orc, ctx, deg):
     cloud = ws.synth.make_cloud(20000, 5)
     pos, rot = ws.synth.orbit_camera(80.0)
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, max_sh_deg=deg)
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, max_sh_deg=deg)
 
 
 def test_options_mip_kernel_scaling_walltime(ws, orc, ctx):
     """§8(f) N4 options: mip-splatting compensation, kernel size, gaussian_scaling, walltime reveal."""
     cloud = ws.synth.make_cloud(20000, 6)
     pos, rot = ws.synth.orbit_camera(10.0)
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, mip_splatting=True, kernel_size=0.1)
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, gaussian_scaling=0.5)
-    _check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, walltime=0.6)       # partially revealed: NaN axes vanish
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, mip_splatting=True, kernel_size=0.1)
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, gaussian_scaling=0.5)
+    check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, walltime=0.6)       # partially revealed: NaN axes vanish
 
 
 def test_options_clipping_box_and_background(ws, orc, ctx):
@@ -159,12 +99,12 @@ def test_options_clipping_box_and_background(ws, orc, ctx):
     cloud = ws.synth.make_cloud(20000, 12)
     pos, rot = ws.synth.orbit_camera(200.0)
     box = ws.Aabb([-0.5, -1.0, -0.25], [0.75, 0.5, 1.0])
-    r, st, _ = _check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, clipping_box=box)
-    full = _frame(ws, ctx, cloud, pos, rot, 400, 300)[0].stats()["num_visible"]
+    r, st, _ = check_all_stages(ws, orc, ctx, cloud, pos, rot, 400, 300, clipping_box=box)
+    full = frame(ws, ctx, cloud, pos, rot, 400, 300)[0].stats()["num_visible"]
     assert 0 < st["num_visible"] < full
     bg = (0.2, 0.4, 0.6, 1.0)
-    _, _, on_bg, _ = _frame(ws, ctx, cloud, pos, rot, 400, 300, clear=bg)
-    _, _, on_zero, _ = _frame(ws, ctx, cloud, pos, rot, 400, 300)
+    _, _, on_bg, _ = frame(ws, ctx, cloud, pos, rot, 400, 300, clear=bg)
+    _, _, on_zero, _ = frame(ws, ctx, cloud, pos, rot, 400, 300)
     want = on_zero + (1.0 - on_zero[..., 3:4]) * np.asarray(bg, np.float32)        # src + dst * (1 - src.a)
     assert np.abs(on_bg - want).max() < 2e-6
 
@@ -181,8 +121,8 @@ def test_occlusion_split_is_bit_identical(ws, orc, ctx):
     for cloud, W, H, az, fmt in cases:
         pos, rot = ws.synth.orbit_camera(az)
         clear = (0.1, 0.2, 0.3, 0.4)
-        r0, _, img0, _ = _frame(ws, ctx, cloud, pos, rot, W, H, fmt=fmt, clear=clear, split=False)
-        r1, _, img1, _ = _frame(ws, ctx, cloud, pos, rot, W, H, fmt=fmt, clear=clear, split=True)
+        r0, _, img0, _ = frame(ws, ctx, cloud, pos, rot, W, H, fmt=fmt, clear=clear, split=False)
+        r1, _, img1, _ = frame(ws, ctx, cloud, pos, rot, W, H, fmt=fmt, clear=clear, split=True)
         assert np.array_equal(img0.view(np.uint8), img1.view(np.uint8))
         s0, s1 = r0.stats(), r1.stats()
         assert s1["num_visible"] == s0["num_visible"] and s1["num_pairs"] <= s0["num_pairs"]
@@ -212,17 +152,17 @@ def test_edge_cases(ws, orc, ctx):
     pos, rot = ws.synth.fixed_camera()
     # empty cloud
     c0 = ws.synth.make_cloud(0, 1)
-    r, pc, img, _ = _frame(ws, ctx, c0, pos, rot, 64, 48, clear=(0.25, 0.5, 0.75, 1.0))
+    r, pc, img, _ = frame(ws, ctx, c0, pos, rot, 64, 48, clear=(0.25, 0.5, 0.75, 1.0))
     assert r.num_visible_points() == 0 and r.stats()["num_pairs"] == 0
     assert np.allclose(img, (0.25, 0.5, 0.75, 1.0))
     # everything culled (camera looks away)
     c1 = ws.synth.make_cloud(3000, 2)
-    r, pc, img, _ = _frame(ws, ctx, c1, np.array([0, 0, 3], np.float32), rot, 64, 48)
+    r, pc, img, _ = frame(ws, ctx, c1, np.array([0, 0, 3], np.float32), rot, 64, 48)
     assert r.num_visible_points() == 0 and np.count_nonzero(img) == 0
     # one huge splat covering every tile + a few small ones
     c2 = ws.synth.make_cloud(300, 3)
     c2["gaussians"]["cov"][0] = np.array([4, 0.01, 0, 4, 0, 4], np.float16)
-    _check_all_stages(ws, orc, ctx, c2, pos, rot, 330, 250)
+    check_all_stages(ws, orc, ctx, c2, pos, rot, 330, 250)
 
 
 def test_output_formats(ws, orc, ctx):
@@ -230,9 +170,9 @@ def test_output_formats(ws, orc, ctx):
     pos, rot = ws.synth.orbit_camera(300.0)
     W, H = 400, 300
     clear = (0.1, 0.2, 0.3, 1.0)
-    _, _, f32, _ = _frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA32_FLOAT, clear)
-    _, _, f16, _ = _frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA16_FLOAT, clear)
-    _, _, u8, _ = _frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA8_UNORM, clear)
+    _, _, f32, _ = frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA32_FLOAT, clear)
+    _, _, f16, _ = frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA16_FLOAT, clear)
+    _, _, u8, _ = frame(ws, ctx, cloud, pos, rot, W, H, ws.FORMAT_RGBA8_UNORM, clear)
     assert np.array_equal(f16, f32.astype(np.float16))
     assert np.array_equal(u8, np.rint(np.clip(f32, 0, 1) * 255).astype(np.uint8))
 
@@ -288,7 +228,7 @@ def test_determinism(ws, ctx):
     """Bit-reproducible frames (the reference's atomic slot order is not, preprocess.wgsl:262)."""
     cloud = ws.synth.make_cloud(30000, 8)
     pos, rot = ws.synth.orbit_camera(120.0)
-    imgs = [_frame(ws, ctx, cloud, pos, rot, 512, 288)[2] for _ in range(3)]
+    imgs = [frame(ws, ctx, cloud, pos, rot, 512, 288)[2] for _ in range(3)]
     assert np.array_equal(imgs[0], imgs[1]) and np.array_equal(imgs[0], imgs[2])
 
 
@@ -298,7 +238,7 @@ def _check_compressed(ws, orc, ctx, cloud, pos, rot, W, H, **kw):
     scale factor differs between glibc and CUDA by an ulp, which propagates into the axes); the
     image is compared against the oracle composited over the CUDA splats' own order."""
     from helpers import f16_ordered
-    r, pc, img, (fovx, fovy) = _frame(ws, ctx, cloud, pos, rot, W, H, **kw)
+    r, pc, img, (fovx, fovy) = frame(ws, ctx, cloud, pos, rot, W, H, **kw)
     zn, zf = orc.fit_near_far(pos, cloud["aabb_min"], cloud["aabb_max"])
     cam = orc.camera_uniform(pos, rot, fovx, fovy, zn, zf, W, H)
     st = orc.render_settings(cloud, **kw)
@@ -390,7 +330,7 @@ def test_analytic_isotropic_gaussian_on_cuda_path(ws, ctx):
                  aabb_max=np.array([1, 1, 1], np.float32), center=np.zeros(3, np.float32))
     pos, rot = ws.synth.fixed_camera()
     for split in (False, True):
-        r, pc, img, _ = _frame(ws, ctx, cloud, pos, rot, W, H, split=split)
+        r, pc, img, _ = frame(ws, ctx, cloud, pos, rot, W, H, split=split)
         assert r.num_visible_points() == 1
         f = H / (2 * math.tan(fovy / 2))
         var = (f * sigma / 3.0) ** 2 + 0.3
@@ -414,7 +354,7 @@ def test_cuda_image_against_independent_f64_renderer(ws, ctx, az):
     cloud = ws.synth.make_cloud(n, 99)
     pos, rot = ws.synth.orbit_camera(az)
     clear = (0.1, 0.2, 0.3, 1.0)
-    r, pc, img, (fovx, fovy) = _frame(ws, ctx, cloud, pos, rot, W, H, clear=clear)
+    r, pc, img, (fovx, fovy) = frame(ws, ctx, cloud, pos, rot, W, H, clear=clear)
     zn, zf = orc.fit_near_far(pos, cloud["aabb_min"], cloud["aabb_max"])
     ideal, idx = f64_ideal.render(cloud, pos, rot, W, H, fovx, fovy, zn, zf, clear=clear)
     assert len(idx) == r.num_visible_points()
@@ -437,11 +377,11 @@ def test_target_formats_against_rop_faithful_oracle(ws, orc, ctx):
     fovx, fovy = ws.synth.fov_for_viewport(W, H)
     ref = orc.render_frame(cloud, pos, rot, W, H, fovx, fovy)
     assert ref["splats"][:, 6:9].view(np.float16).max() <= 1.0
-    r8, _, img8, _ = _frame(ws, ctx, cloud, pos, rot, W, H, fmt=ws.FORMAT_RGBA8_UNORM, split=True)
+    r8, _, img8, _ = frame(ws, ctx, cloud, pos, rot, W, H, fmt=ws.FORMAT_RGBA8_UNORM, split=True)
     rop8 = orc.composite_rop(ref["splats"], ref["order"], W, H, 0)
     gap8 = np.abs(img8.astype(np.float32) / 255.0 - rop8).max(axis=2)
     assert gap8.max() <= 8.0 / 255.0 + 1e-6 and gap8.mean() <= 1.5 / 255.0, (gap8.max() * 255, gap8.mean() * 255)
-    r16, _, img16, _ = _frame(ws, ctx, cloud, pos, rot, W, H, fmt=ws.FORMAT_RGBA16_FLOAT, split=True)
+    r16, _, img16, _ = frame(ws, ctx, cloud, pos, rot, W, H, fmt=ws.FORMAT_RGBA16_FLOAT, split=True)
     rop16 = orc.composite_rop(ref["splats"], ref["order"], W, H, 1)
     rel = np.abs(img16.astype(np.float32) - rop16).max(axis=2) / np.maximum(np.abs(rop16).max(axis=2), 2.0 ** -10)
     assert rel.max() < 6e-3 + 2e-3 and rel.mean() < 1e-3, (rel.max(), rel.mean())
@@ -483,7 +423,7 @@ def test_deferred_frame_status_and_index_validation(ws, ctx):
         ws.PointCloud.new(ctx, make_generic(ws, bad))
     ws.PointCloud.new(ctx, make_generic(ws, cc))             # the untouched cloud loads
     # (3) a second context on the same device (and on device 1 when there is one) renders the same frame
-    img0 = _frame(ws, ctx, cloud, pos, rot, 320, 200)[2]
+    img0 = frame(ws, ctx, cloud, pos, rot, 320, 200)[2]
     for dev in range(min(torch.cuda.device_count(), 2)):
         ctx2 = ws.Context(dev)
         with torch.cuda.device(dev):
@@ -505,5 +445,5 @@ def test_binning_large_rectangles(ws, orc, ctx, scaling, n, W, H):
     (gaussian_scaling blows the splats up: hundreds to thousands of tiles each, screen-filling ones included)."""
     cloud = ws.synth.make_cloud(n, 123 + n)
     pos, rot = ws.synth.orbit_camera(300.0)
-    r, st, d = _check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H, gaussian_scaling=scaling)
+    r, st, d = check_all_stages(ws, orc, ctx, cloud, pos, rot, W, H, gaussian_scaling=scaling)
     assert st["num_pairs"] > (20 * st["num_visible"] if scaling > 1 else st["num_visible"])

@@ -629,8 +629,8 @@ class GaussianRenderer:
     def prepare(self, stream, pc, render_settings):
         """Enqueue stage 1 + 2 on `stream` (torch.cuda.Stream, raw cudaStream_t int, or None)."""
         a = render_settings._c()
-        self._viewport = render_settings.viewport
         _check(lib().ws_renderer_prepare(self._h, pc._h, C.byref(a), _stream_handle(stream)))
+        self._viewport = render_settings.viewport       # a rejected frame leaves the prepared one (and its row pitch) in place
 
     def render(self, target, pc, clear=(0.0, 0.0, 0.0, 0.0), stream=None, row_pitch=None):
         """Enqueue stage 3 into `target`: a device pointer (int) or an object with .data_ptr()

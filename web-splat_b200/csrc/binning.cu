@@ -195,6 +195,7 @@ bin_scan_kernel(BinningArgs a)
     if (threadIdx.x == 0) {
         const uint64_t P = (nparts > 0u) ? total_out : 0ull;           // 64-bit: screen-filling splats can push P past 2^32
         *a.num_pairs_out = P > 0xffffffffull ? 0xffffffffu : (uint32_t)P;
+        *a.num_pairs64_out = P;
         if (P > (uint64_t)a.pair_cap) a.counters->pair_overflow = 1u;  // zeroed per frame; either slab may set it
     }
 }
@@ -386,7 +387,9 @@ bin_expand_v1_kernel(BinningArgs a)
             // m >= 2^32/w with m*w - 2^32 <= w + 512: floor(t/w) == umulhi(t, m) for every t < 2^20, w <= 1024 (viewport <= 16384)
         }
 
-        for (uint32_t c0 = 0; c0 < total; c0 += BIN_CAP) {
+        // (a chunk that starts at or past the capacity stores nothing: stop there -- an overflowing partition of
+        // screen-filling splats would otherwise walk up to 2^30 positions for nothing)
+        for (uint32_t c0 = 0; c0 < total && (uint64_t)base + c0 < cap; c0 += BIN_CAP) {
             const uint32_t m = (total - c0 < (uint32_t)BIN_CAP) ? total - c0 : (uint32_t)BIN_CAP;
             const uint32_t rounds = (m + BIN_THREADS - 1u) / BIN_THREADS;       // 32-position rounds per warp
             const uint32_t span = rounds * 32u;                                 // consecutive positions owned by a warp

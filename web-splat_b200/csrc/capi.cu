@@ -1108,12 +1108,14 @@ static ws_status enqueue_stage2(ws_renderer *r, cudaStream_t stream)
         const size_t set_off = half ? 3 * sparts_p : 0, gset_off = half ? 3 * gparts_p : 0;
         const uint32_t cap = r->pair_cap;
         uint32_t *num_pairs = (r->frame_split && !half) ? &r->d_counters->num_pairs_near : &r->d_counters->num_pairs;
+        uint64_t *num_pairs64 = (r->frame_split && !half) ? &r->d_counters->num_pairs_near64 : &r->d_counters->num_pairs64;
         {
             BinningArgs a;
             a.sorted_slots = sorted_slots; a.list_len = list_len ? list_len : &r->d_counters->num_visible; a.rects = r->d_rects; a.uniforms = r->d_uniforms;
             a.counters = r->d_counters; a.pair_tiles = r->d_ptiles[0]; a.pair_slots = r->d_pslots[0];
             a.part_counts = r->d_scan_bin; a.part_bases = r->d_bin_bases; a.hist = r->d_hist_tile + half * 4 * 256;
             a.slab = slab; a.tile_done = (slab == 2u) ? r->d_tile_done : nullptr; a.pair_cap = cap; a.num_pairs_out = num_pairs;
+            a.num_pairs64_out = num_pairs64;
             a.keep4 = r->d_keep4;
             a.num_tiles_hint = r->h_uniforms.tiles_x * r->h_uniforms.tiles_y; a.done_in_smem = 0;
             a.near_pct = split_near_pct();
@@ -1756,7 +1758,7 @@ extern "C" ws_status ws_renderer_stats(ws_renderer *r, ws_frame_stats *s)
     for (int i = 0; i < ws_renderer::FLAG_SLOTS; i++) r->flags_pending[i] = false;   // this call reports the frame's status itself
     const FrameUniforms &U = r->h_uniforms;
     s->num_points = r->last_n; s->num_visible = c.num_visible;
-    s->num_pairs = (uint64_t)c.num_pairs + (r->frame_split ? c.num_pairs_near : 0u);      // split frames: near slab + what the far slab still had to emit
+    s->num_pairs = c.num_pairs64 + (r->frame_split ? c.num_pairs_near64 : 0u);          // split frames: near slab + what the far slab still had to emit
     s->pair_capacity = r->pair_cap; s->num_tiles = U.tiles_x * U.tiles_y; s->width = U.width; s->height = U.height;
     if (r->timing) {
         auto el = [&](int a, int b) { float ms = 0.f; return (cudaEventElapsedTime(&ms, r->ev[a], r->ev[b]) == cudaSuccess) ? ms : 0.f; };

@@ -63,6 +63,10 @@ struct FrameCounters {
     uint32_t num_far;           // far splats that survive the cull against the saturated tiles
     uint32_t cut_done;          // CTAs of the cut histogram that have finished (the last one picks the cut)
     uint32_t ticket_far[4];     // depth passes over the far survivors
+    // exact pair totals (bin_scan_kernel): P can pass 2^32 (screen-filling splats at 16 K viewports), where the 32-bit
+    // num_pairs / num_pairs_near above saturate at 0xffffffff -- those stay 32-bit, the tile-sort passes read them as n_ptr
+    uint64_t num_pairs64;       // P of the only slab, or of the far slab of a split frame
+    uint64_t num_pairs_near64;  // occlusion split: P of the near slab
 };
 
 constexpr int TILE = 16;                    // 16x16 pixel tiles

@@ -71,7 +71,8 @@ struct BinningArgs {
     const uint8_t *tile_done;     // slab 2: tiles already saturated by the near slab; a splat whose whole rectangle is done emits no pair
     uint32_t *keep4;              // slab 2: ceil(V/2/4) words, one byte per splat: count kernel -> expand kernel
     uint32_t pair_cap;            // capacity of pair_tiles / pair_slots for this launch
-    uint32_t *num_pairs_out;      // device counter that receives the number of pairs of this launch
+    uint32_t *num_pairs_out;      // device counter that receives the number of pairs of this launch (saturated at 0xffffffff)
+    uint64_t *num_pairs64_out;    // ... and the exact 64-bit count (ws_renderer_stats)
     uint32_t near_pct;            // occlusion split: share of the depth-sorted splats in the near slab, in percent (0 = the default quarter)
     uint32_t num_tiles_hint;      // host-known number of tiles (sizes the shared-memory copy of tile_done); 0 = unknown
     uint32_t done_in_smem;        // set by launch_binning
